@@ -2,9 +2,9 @@
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--views V] [--impl ours|reference|library]
 
-* ours, 1 GPU: BASELINE.json configs[1] (N=32 views, 512x368, bf16 tensor-core operands) on one B200 is the
+* ours, 1 GPU: BASELINE.json configs[1] (N=32 views, 512x368, bf16 tensor-core operands) on one H100 is the
   headline `value`; `config.extra` adds configs[2] (N=320, long-sequence regime) with its own roofline, the
-  per-GEMM rates of the fusion-decoder linears, and the "library bar" (the UNMODIFIED reference model on the same B200
+  per-GEMM rates of the fusion-decoder linears, and the "library bar" (the UNMODIFIED reference model on the same GPU
   under bf16 autocast + SDPA-flash, from oracle/_ref).
 * ours, N GPUs (torchrun, one rank per GPU): the SAME total N=32 workload, views sharded by contiguous ranges
   (sequence-parallel fusion decoder, K|V exchange per layer over NCCL) -> "scaling": "strong"; `config.extra` adds the
@@ -15,6 +15,10 @@
 
 One JSON line on stdout (rank 0).  `value` = views/s with inputs resident in HBM; `e2e` = the same metric through
 the reference-facing API `inference()` from pinned host buffers including H2D and D2H.
+
+--dump-outputs DIR writes the predictions of the last timed step (rank 0's views) as DIR/<key>.npy, float32, shape
+(views, DUMP_PIXELS, channels): the same seeded sample of pixel positions for every view and run, so that two builds
+can be compared output for output (the inputs and weights are seeded, hence identical between runs).
 """
 import argparse
 import json
@@ -43,8 +47,9 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json, sustained)"
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3) for a card allowed 700 W: an upper bound, not a reached rate
+    return 989.0, 3350.0, "H100 SXM data sheet (700 W)"
 
 
 class ClockSampler:
@@ -240,7 +245,7 @@ def run_reference(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
-# ----------------------------------------------------------------------------- library bar (reference on the B200)
+# ----------------------------------------------------------------------------- library bar (reference on this GPU)
 def library_bar(n_views, dev, steps=3, warmup=2):
     """The UNMODIFIED reference model on this GPU: bf16 autocast + SDPA-flash (BASELINE.md §4 item 4) - torch/cuBLAS/
     cuDNN/flash kernels, none of ours.  Returns a dict (or {"unavailable": why})."""
@@ -272,7 +277,7 @@ def library_bar(n_views, dev, steps=3, warmup=2):
         torch.cuda.empty_cache()
         return {"views": n_views, "ms_per_forward": ms, "views_per_sec": n_views / (ms * 1e-3),
                 "achieved_tflops_whole_forward": flops_total(n_views) / (ms * 1e-3) / 1e12,
-                "what": "reference Fast3R.forward (oracle/_ref) on this B200, torch.autocast(bfloat16), "
+                "what": "reference Fast3R.forward (oracle/_ref) on this GPU, torch.autocast(bfloat16), "
                         "attn_implementation=flash_attention (SDPA flash), device-resident inputs"}
     except Exception as e:  # the bar is context, never a reason to lose the headline number
         torch.cuda.empty_cache()
@@ -434,14 +439,40 @@ def attention_roofline(timer, n_views, ms_step, clocks, peak_tf, peak_src):
             "traffic": None,
             "algorithmic_bytes_per_launch": 2.0 * DMODEL * (2 * sq + 2 * n_views * P_TOK),
             "share_of_step": DEPTH * att_ms / ms_step}
-    try:  # the binding unit at head_dim 64 is the special-function unit (16 ex2 / clk / SM)
-        clk = (clocks or {}).get("sm_mhz") or 1965.0
+    try:  # at head_dim 64 the special-function unit (16 ex2 / clk / SM) is the other candidate bound
+        import torch
+        sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+        clk = (clocks or {}).get("sm_mhz") or (clocks or {}).get("sm_max_mhz") or 1980.0
         exps = float(sq) * (n_views * P_TOK) * (DMODEL // 64)
-        roof["sfu"] = {"exp2_per_launch": exps, "peak_exp2_per_s": 148 * 16 * clk * 1e6,
-                       "frac": exps / (att_ms * 1e-3) / (148 * 16 * clk * 1e6), "sm_mhz": clk}
+        roof["sfu"] = {"exp2_per_launch": exps, "peak_exp2_per_s": sms * 16 * clk * 1e6,
+                       "frac": exps / (att_ms * 1e-3) / (sms * 16 * clk * 1e6), "sm_mhz": clk}
     except Exception:
         pass
     return roof, att_ms
+
+
+DUMP_PIXELS = 32768  # sampled pixel positions per view: 32 views x 8 channels in all x 4 B x 32768 = 32 MB
+
+
+def dump_outputs(out_dir, preds):
+    """preds: list (one dict per view) of the forward's outputs; writes one float32 array per key."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    views = [p for p in preds if p]
+    if not views:
+        return
+    for key in sorted(views[0]):
+        t0 = views[0][key]
+        if not torch.is_tensor(t0) or not t0.is_floating_point():
+            continue
+        # (1, H, W[, C]) per view -> (H*W, C)
+        per_view = [p[key].detach().float().reshape(t0.shape[1] * t0.shape[2], -1) for p in views]
+        n_pix = per_view[0].shape[0]
+        g = torch.Generator().manual_seed(0)
+        idx = torch.randperm(n_pix, generator=g)[:DUMP_PIXELS].sort().values
+        arr = torch.stack([v[idx.to(v.device)] for v in per_view]).cpu().numpy().astype(np.float32)
+        np.save(os.path.join(out_dir, f"{key}.npy"), arr)
 
 
 def run_ours(args, rank, world, local_rank):
@@ -473,7 +504,8 @@ def run_ours(args, rank, world, local_rank):
         return [float(x) for x in t]
 
     def timed_device(views, steps, warmup):
-        """K forwards with device-resident inputs; returns (ms/step max over ranks, launches, attention timer)."""
+        """K forwards with device-resident inputs; returns (ms/step max over ranks, launches, attention timer,
+        predictions of the last step)."""
         def step():
             torch.manual_seed(7)
             return model(views)
@@ -485,13 +517,14 @@ def run_ours(args, rank, world, local_rank):
         n0 = L.launch_count()
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        preds = None
         e0.record()
         for _ in range(steps):
-            step()
+            preds = step()
         e1.record()
         barrier()
         ops.KERNEL_TIMER = None
-        return e0.elapsed_time(e1) / steps, L.launch_count() - n0, timer
+        return e0.elapsed_time(e1) / steps, L.launch_count() - n0, timer, preds
 
     # ================= headline: N = args.views (default 32, BASELINE configs[1]) =================
     N = args.views
@@ -508,8 +541,11 @@ def run_ours(args, rank, world, local_rank):
     sampler.mark()
     if sp is not None:
         sp.timers = []
-    ms, launches, timer = timed_device(views_dev, args.steps, 0)
+    ms, launches, timer, preds = timed_device(views_dev, args.steps, 0)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, preds)
+    del preds
     roof, att_ms = attention_roofline(timer, N, ms, clocks, peak_tf, peak_src)
     sp_trace = None
     if sp is not None and sp.timers:
@@ -589,7 +625,8 @@ def run_ours(args, rank, world, local_rank):
         vd = make_views(n_views, device=dev, only=r)
         if sp is not None:
             sp.timers = []
-        m, _l, tm = timed_device(vd, steps, warmup)
+        m, _l, tm, _p = timed_device(vd, steps, warmup)
+        del _p
         rf, am = attention_roofline(tm, n_views, m, clocks, peak_tf, peak_src)
         if sp is not None and sp.timers:   # sharded: the attention of a layer = key-range partials + merge (+ exposed wait)
             tr, sp.timers = sp.timers[-DEPTH * steps:], None
@@ -634,7 +671,7 @@ def run_ours(args, rank, world, local_rank):
                                    "random-init weights, fp32 pointmaps out",
                        "views": N, "tokens": N * P_TOK,
                        "parallelism": "single GPU" if world == 1 else f"sequence-parallel x{world} (K|V exchange/layer)",
-                       "l2": "working set (1.3 GB weights + GBs of activations per step) exceeds the 126 MB L2; no explicit flush",
+                       "l2": "working set (1.3 GB weights + GBs of activations per step) exceeds the 50 MB L2; no explicit flush",
                        "achieved_tflops_whole_forward": flops_total(N) / (ms * 1e-3) / 1e12,
                        "extra": extra},
             "clocks": clocks, "gpu_launches": int(launches),
@@ -660,6 +697,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip config.extra (N=320 / N=1000 / GEMM rates / library bar)")
     ap.add_argument("--no-library-bar", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the predictions of the last timed step as DIR/<key>.npy (seeded pixel sample)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -669,7 +708,7 @@ def main():
         return
     import torch
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py --impl ours needs a B200 (no CPU fallback); use --impl reference for the CPU arm")
+        raise SystemExit("bench.py --impl ours needs a CUDA GPU (no CPU fallback); use --impl reference for the CPU arm")
     if args.impl == "library":
         run_library(args, rank, world, local_rank)
         return

@@ -1,4 +1,4 @@
-"""fast3r_b200 — B200-native (sm_100a) implementation of the Fast3R single-forward-pass hot path.
+"""fast3r_b200 — H100-native (sm_90a) implementation of the Fast3R single-forward-pass hot path.
 
 Public surface mirrors the reference: ``Fast3R`` (fast3r/models/fast3r.py:45) and ``inference`` /
 ``loss_of_one_batch`` (fast3r/dust3r/inference_multiview.py).  The compute lives in ``libfast3r_b200.so``

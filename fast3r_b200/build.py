@@ -1,4 +1,4 @@
-"""Builds libfast3r_b200.so (sm_100a only) in-tree with nvcc.  No GPU needed (cross-compile)."""
+"""Builds libfast3r_b200.so (sm_90a only) in-tree with nvcc.  No GPU needed (cross-compile)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfast3r_b200.so")
 SOURCES = ["capi.cu", "gemm.cu", "attention.cu", "attention_x3.cu", "elementwise.cu", "ingest.cu", "geometry.cu"]
 HEADERS = ["common.cuh", "f3r_kernels.h", "geometry_math.h", os.path.join("..", "..", "include", "fast3r_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC"]
 
 

@@ -1,10 +1,10 @@
-"""Making the reference code base use the B200 model unchanged.
+"""Making the reference code base use this model unchanged.
 
 `MultiViewDUSt3RLitModule.forward(views)` is literally ``self.net(views)`` and `load_for_inference(net)` only stores
 `net` (fast3r/models/multiview_dust3r_module.py:119-126), so an instance of ``fast3r_b200.Fast3R`` can be handed to it
 directly.  The one place that looks at the class is ``isinstance(self.net, Fast3R)`` when pretrained weights are loaded
 (multiview_dust3r_module.py:1005): `install()` rebinds the name ``fast3r.models.fast3r.Fast3R`` (and the copy already
-imported into the Lightning module, if any) to the B200 class, so that check - and Hydra configs whose ``_target_`` is
+imported into the Lightning module, if any) to this package's class, so that check - and Hydra configs whose ``_target_`` is
 ``fast3r.models.fast3r.Fast3R`` - resolve to this implementation.  Call it once, before building the Lightning module."""
 import importlib
 import sys

@@ -1,32 +1,21 @@
-// FlashAttention-style forward for head_dim 64 on sm_100a: softmax(scale * Q K^T) V, non-causal, no mask
+// FlashAttention-style forward for head_dim 64 on sm_90a: softmax(scale * Q K^T) V, non-causal, no mask
 // (fast3r/croco/models/blocks.py:135-194; encoder: batch = views, S = P; fusion decoder: batch = B, S = N*P).
 //
-// One CTA owns 256 query rows (two 128-row tiles that ping-pong) of one (batch, head) and streams all keys
-// in blocks of 128.  K/V blocks arrive by TMA into a 128B-swizzled smem ring shared by both tiles;
-// S = Q K^T and O += P V run on tcgen05 with S, P and O all resident in TMEM (512 columns:
-// S0 S1 | P0 P1 | O0 O1).  P is written back to TMEM as packed bf16 and consumed as the TMEM A-operand of the
-// PV MMA, V is consumed as an MN-major smem B operand, so no transposes or smem round trips are needed.
-// Softmax is exact online softmax in fp32 (exp2 domain) with lazy O rescaling: the running reference max is
-// only moved when the row max grows by more than 2^8, which makes the TMEM read-modify-write of O rare.
-//
-// Warp roles: warp 0 = TMA producer, warps 1 / 2 = MMA issuers of tile 0 / 1 (one elected thread each), warps 4-7 = softmax of tile 0,
-// warps 8-11 = softmax of tile 1 (one thread per query row).  setmaxnreg moves registers from warpgroup 0
-// to the softmax warpgroups, which keep a whole 128-wide score row in registers.
-#include <cstdlib>
-
+// One CTA owns 128 query rows of one (batch, head) and streams all keys of its range in blocks of 128.  Warpgroup 0
+// is the TMA producer (Q once, K/V blocks into a 128B-swizzled smem ring); warpgroups 1 and 2 each own 64 query rows:
+// S = Q K^T is a wgmma with both operands in shared memory (S stays in registers), P is packed to bf16 in registers
+// and used directly as the register A operand of O += P V (V consumed MN-major from shared memory, no transpose).
+// Softmax is exact online softmax in fp32 (exp2 domain) with lazy O rescaling: the running reference max is only
+// moved when the row max grows by more than 2^8.
 #include "common.cuh"
 #include "f3r_kernels.h"
 
 namespace f3r {
 
-// kSplit = softmax threads per query row: 1 (8 softmax warps, a whole 128-wide score row per thread) or 2 (16 softmax
-// warps = 4 per scheduler, 64 columns per thread: more warps to hide the fixed-latency stalls of the exp2 chains)
-template <int kSplit> constexpr int att_threads() { return 128 + 256 * kSplit; }  // warpgroup 0: TMA + 2 MMA issuers
-constexpr int ATT_STAGES = 4;
+constexpr int ATT_THREADS = 384;
+constexpr int ATT_STAGES = 3;
 constexpr int ATT_TILE_BYTES = 128 * 64 * 2;  // 16 KB: 128 rows x 64 bf16
-constexpr int ATT_SMEM_BYTES = (2 + 2 * ATT_STAGES) * ATT_TILE_BYTES + 1024 + 256 + 4096 /*half-row exchange*/;
-
-constexpr uint32_t TM_S0 = 0, TM_S1 = 128, TM_P0 = 256, TM_P1 = 320, TM_O0 = 384, TM_O1 = 448;
+constexpr int ATT_SMEM_BYTES = (1 + 2 * ATT_STAGES) * ATT_TILE_BYTES + 1024 + 256;
 
 F3R_DEVICE float ex2_approx(float x) {
   float y;
@@ -34,70 +23,13 @@ F3R_DEVICE float ex2_approx(float x) {
   return y;
 }
 
-// Blackwell packed fp32x2 / 3-input ALU ops (SASS FFMA2 / FADD2 / FMNMX3): halve the issue slots of the softmax.
-F3R_DEVICE float max3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-F3R_DEVICE void ffma2(float& d0, float& d1, float a0, float a1, float b, float c) {
-  asm("{ .reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%4}; mov.b64 rc, {%5,%5};\n\t"
-      "fma.rn.f32x2 rd, ra, rb, rc; mov.b64 {%0,%1}, rd; }"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b), "f"(c));
-}
-F3R_DEVICE void fadd2(float& d0, float& d1, float a0, float a1) {
-  asm("{ .reg .b64 ra, rd; mov.b64 rd, {%0,%1}; mov.b64 ra, {%2,%3};\n\t"
-      "add.rn.f32x2 rd, rd, ra; mov.b64 {%0,%1}, rd; }"
-      : "+f"(d0), "+f"(d1) : "f"(a0), "f"(a1));
-}
-
-// exp2 of a PAIR on the FMA / ALU pipes instead of the special-function unit (MUFU.EX2 issues 16 / clk / SM, which at
-// head_dim 64 is the binding unit of this kernel: 2 x 128 x 128 exponentials per key block = 2048 clk vs 1024 clk of
-// MMA).  Cody-Waite split x = n + f with a magic-number add (round to nearest, f in [-0.5, 0.5]), degree-3 minimax
-// polynomial of 2^f (max rel. error 7.6e-5, well below the bf16 rounding of P: 2e-3), exponent patched in with an
-// integer shift-add.  6 packed FMA-pipe instructions + 4 ALU instructions per pair against 2 MUFU (16 clk of XU time).
-// x is clamped at -126 (2^-126 ~ 0); the lazy-rescale rule bounds x from above by 8.
-F3R_DEVICE void exp2_emu2(float& e0, float& e1, float x0, float x1) {
-  uint32_t t0, t1, p0, p1;
-  asm("{ .reg .b64 x, t, r, f, p, k;\n\t"
-      ".reg .f32 xa, xb;\n\t"
-      "max.f32 xa, %4, 0fC2FC0000;\n\t"            // -126.0
-      "max.f32 xb, %5, 0fC2FC0000;\n\t"
-      "mov.b64 x, {xa, xb};\n\t"
-      "mov.b64 k, {%6, %6};\n\t"
-      "add.rn.f32x2 t, x, k;\n\t"                  // t = x + 1.5*2^23: low mantissa bits hold round(x)
-      "sub.rn.f32x2 r, t, k;\n\t"                  // r = round(x)
-      "sub.rn.f32x2 f, x, r;\n\t"                  // f = x - r in [-0.5, 0.5]
-      "mov.b64 k, {%7, %7};\n\t"
-      "mov.b64 p, {%8, %8};\n\t"
-      "fma.rn.f32x2 p, f, k, p;\n\t"               // c3 f + c2
-      "mov.b64 k, {%9, %9};\n\t"
-      "fma.rn.f32x2 p, p, f, k;\n\t"               // .. f + c1
-      "mov.b64 k, {%10, %10};\n\t"
-      "fma.rn.f32x2 p, p, f, k;\n\t"               // .. f + c0
-      "mov.b64 {%0, %1}, t;\n\t"
-      "mov.b64 {%2, %3}, p; }"
-      : "=r"(t0), "=r"(t1), "=r"(p0), "=r"(p1)
-      : "f"(x0), "f"(x1), "f"(12582912.f), "f"(0.05520550534f), "f"(0.2426139712f), "f"(0.6932547688f),
-        "f"(0.9999276996f));
-  e0 = __uint_as_float(p0 + (t0 << 23));
-  e1 = __uint_as_float(p1 + (t1 << 23));
-}
-
-// kEmu of every 8 score pairs take the FMA-pipe exp2 (0: all on MUFU).  Spread patterns keep each group of four
-// consecutive pairs mixed so that the scheduler can interleave the two instruction streams.
-template <int kEmu> __host__ __device__ constexpr uint32_t emu_mask() {
-  return kEmu == 0 ? 0x00u : kEmu == 1 ? 0x10u : kEmu == 2 ? 0x44u : 0x92u;
-}
-
-template <int kEmu, int kSplit>
-__global__ void __launch_bounds__(att_threads<kSplit>(), 1)
+__global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
                  const __grid_constant__ AttnArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_q = smem;                                   // 2 tiles
-  uint8_t* smem_k = smem + 2 * ATT_TILE_BYTES;              // ATT_STAGES tiles
+  uint8_t* smem_q = smem;                                   // 1 tile
+  uint8_t* smem_k = smem + ATT_TILE_BYTES;                  // ATT_STAGES tiles
   uint8_t* smem_v = smem_k + ATT_STAGES * ATT_TILE_BYTES;   // ATT_STAGES tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_v + ATT_STAGES * ATT_TILE_BYTES);
   uint64_t* q_full = bars;                       // 1
@@ -105,17 +37,11 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   uint64_t* k_empty = k_full + ATT_STAGES;
   uint64_t* v_full = k_empty + ATT_STAGES;
   uint64_t* v_empty = v_full + ATT_STAGES;
-  uint64_t* s_full = v_empty + ATT_STAGES;       // 2
-  uint64_t* s_free = s_full + 2;                 // 2
-  uint64_t* p_full = s_free + 2;                 // 2
-  uint64_t* pv_done = p_full + 2;                // 2
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(pv_done + 2);
-  float* xbuf = reinterpret_cast<float*>(smem_v + ATT_STAGES * ATT_TILE_BYTES + 256);  // [tile][parity][half][128]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // work item = (unit = (batch, head, 256-row query tile), split = slice of the key blocks of this launch's key range)
+  // work item = (unit = (batch, head, 128-row query tile), split = slice of the key blocks of this launch's key range)
   const int unit = blockIdx.x / p.n_split;
   const int split = blockIdx.x % p.n_split;
   const int qt = unit % p.q_tiles;
@@ -132,34 +58,21 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     tma_prefetch_desc(&tmap_kv);
     mbar_init(q_full, 1);
     for (int s = 0; s < ATT_STAGES; ++s) {
-      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 2);  // released by the MMA issuers of both tiles
+      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 2);  // released by both consumer warpgroups
       mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 2);
-    }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&s_full[t], 1); mbar_init(&s_free[t], 128 * kSplit);
-      mbar_init(&p_full[t], 128 * kSplit); mbar_init(&pv_done[t], 1);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   pdl_wait();                // q / kv come from the preceding QKV GEMM: no global access above this line
   pdl_launch_dependents();
 
   if (warp < 4) {
-    // register budget (must balance inside the CTA's launch allocation):
-    //   kSplit 1: 384 thr x 168 = 64512 = 128 x 72 + 256 x 216      kSplit 2: 640 thr x 96 = 61440 = 128 x 64 + 512 x 104
-    if constexpr (kSplit == 1) asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-    else asm volatile("setmaxnreg.dec.sync.aligned.u32 64;");
-  if (warp == 0) {
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");   // 128 x 40 + 256 x 232 <= 64K registers
+    if (warp == 0 && lane == 0) {
       // ===================== TMA producer =====================
-      mbar_arrive_expect_tx(q_full, 2 * ATT_TILE_BYTES);
-      tma_load_3d(smem_q, &tmap_q, q_full, h * 64, qt * 256, b);
-      tma_load_3d(smem_q + ATT_TILE_BYTES, &tmap_q, q_full, h * 64, qt * 256 + 128, b);
+      mbar_arrive_expect_tx(q_full, ATT_TILE_BYTES);
+      tma_load_3d(smem_q, &tmap_q, q_full, h * 64, qt * 128, b);
       int stage = 0; uint32_t phase = 0;
       for (int j = 0; j < nkv; ++j) {
         mbar_wait_relaxed(&k_empty[stage], phase ^ 1);
@@ -172,277 +85,137 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         if (++stage == ATT_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1 || warp == 2) {
-    if (lane == 0) {
-      // ===================== MMA issuers: warp 1 drives query tile 0, warp 2 query tile 1 =====================
-      // One issuing thread PER TILE: S_t(j+1) goes out as soon as the softmax warps of tile t hold S_t(j) in registers
-      // (s_free), independently of the other tile's P (with a single in-order issuer S_1(j+1) queued behind the wait for
-      // P_0(j) and the softmax warps spent 20 % of their time waiting for scores - ncu, profiles/r02_notes.md).
-      const int t = warp - 1;
-      constexpr uint32_t idesc_qk = make_idesc_bf16(128, 128, 0, 0);  // S[128x128] = Q[128x64] K^T, both K-major
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, 0, 1);   // O[128x64] += P[128x128] V, V MN-major
-      const uint64_t qd = make_smem_desc_sw128(smem_u32(smem_q + t * ATT_TILE_BYTES), 1);
-      const uint32_t tm_s = tmem_base + (t ? TM_S1 : TM_S0), tm_p = tmem_base + (t ? TM_P1 : TM_P0);
-      const uint32_t tm_o = tmem_base + (t ? TM_O1 : TM_O0);
-      auto issue_s = [&](int stage) {
-        const uint64_t kdesc = make_smem_desc_sw128(smem_u32(smem_k + stage * ATT_TILE_BYTES), 1);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_ss(tm_s, qd + 2 * k, kdesc + 2 * k, idesc_qk, k > 0 ? 1u : 0u);
-        umma_commit(&s_full[t]);
-        umma_commit(&k_empty[stage]);  // (count 2: both tiles have read this K block)
-      };
-      auto issue_pv = [&](int stage, int j) {
-        const uint64_t vdesc = make_smem_desc_sw128(smem_u32(smem_v + stage * ATT_TILE_BYTES), 0);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)  // 16 keys per MMA: 8 packed-bf16 TMEM columns of P, 16 smem rows (2048 B) of V
-          umma_ts(tm_o, tm_p + 8 * k, vdesc + 128 * k, idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-        umma_commit(&pv_done[t]);
-        umma_commit(&v_empty[stage]);  // (count 2)
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      issue_s(0);
-      for (int j = 0; j < nkv; ++j) {
-        const int st = j % ATT_STAGES;
-        const uint32_t ph = (j / ATT_STAGES) & 1;
-        if (j + 1 < nkv) {
-          const int st1 = (j + 1) % ATT_STAGES;
-          const uint32_t ph1 = ((j + 1) / ATT_STAGES) & 1;
-          mbar_wait(&k_full[st1], ph1);
-          mbar_wait(&s_free[t], j & 1);
-          tc_fence_after();
-          issue_s(st1);
-        }
-        mbar_wait(&v_full[st], ph);
-        mbar_wait(&p_full[t], j & 1);
-        tc_fence_after();
-        issue_pv(st, j);
-      }
-    }
-  }
   } else {
-    // ===================== softmax warps: kSplit threads per query row, 128 / kSplit score columns in registers
-    if constexpr (kSplit == 1) asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-    else asm volatile("setmaxnreg.inc.sync.aligned.u32 104;");
-    constexpr int COLS = 128 / kSplit;      // score columns per thread
-    constexpr int OCOLS = 64 / kSplit;      // output columns per thread
-    const int sw = warp - 4;
-    const int t = sw / (4 * kSplit);        // query tile 0 / 1
-    const int half = (sw >> 2) % kSplit;    // which column slice of the row this thread owns
-    const int quarter = warp & 3;           // TMEM lane quarter accessible to this warp
-    const int row = quarter * 32 + lane;    // row in the 128-row tile
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t tm_s = tmem_base + lane_base + (t ? TM_S1 : TM_S0) + half * COLS;
-    const uint32_t tm_p = tmem_base + lane_base + (t ? TM_P1 : TM_P0) + half * (COLS / 2);
-    const uint32_t tm_o = tmem_base + lane_base + (t ? TM_O1 : TM_O0) + half * OCOLS;
+    // ===================== consumer warpgroups: 64 query rows each =====================
+    // accumulator fragments (common.cuh): this thread holds rows rw + 8 hh (hh = 0, 1) and, in every 8-column group jn,
+    // the columns 8 jn + 2 (lane % 4) + {0, 1}
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cg = (warp - 4) >> 2;
+    const int wg_tid = threadIdx.x & 127;
+    const int rw = cg * 64 + (warp & 3) * 16 + (lane >> 2);  // first of the thread's two rows in the 128-row tile
+    const int cq = 2 * (lane & 3);
     const float sl2 = p.scale_log2;
-    float m_used = -INFINITY;  // raw-score reference max the exponentials are taken against
-    float l = 0.f;             // this thread's (partial) row sum
-    constexpr uint32_t kMask = emu_mask<kEmu>();
+    float m_used[2] = {-INFINITY, -INFINITY};  // raw-score reference max the exponentials are taken against
+    float l[2] = {0.f, 0.f};                   // this thread's partial row sums (its 32 of the 128 columns)
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    const uint64_t qd = make_smem_desc_sw128(smem_u32(smem_q + cg * 64 * 128));
+    mbar_wait(q_full, 0);
 
     for (int j = 0; j < nkv; ++j) {
-      mbar_wait(&s_full[t], j & 1);
-      tc_fence_after();
-      uint32_t s[COLS];
+      const int st = j % ATT_STAGES;
+      const uint32_t ph = (j / ATT_STAGES) & 1;
+      float s[64];
+      mbar_wait(&k_full[st], ph);
+      {
+        const uint64_t kd = make_smem_desc_sw128(smem_u32(smem_k + st * ATT_TILE_BYTES));
+        wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < COLS / 32; ++c) tmem_ld32(tm_s + 32 * c, s + 32 * c);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&s_free[t]);  // S_t may be overwritten by the next QK^T
+        for (int k = 0; k < 4; ++k) wgmma_ss_n128<0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(s);
+      }
+      if (wg_tid == 0) mbar_arrive(&k_empty[st]);
 
       if (j0 + j == nkv_all - 1) {  // last key block of the launch's range: keys past its end are masked
-        const int valid = p.skv - (j0 + j) * 128 - half * COLS;
-        if (valid < COLS) {
+        const int valid = p.skv - (j0 + j) * 128;
+        if (valid < 128) {
 #pragma unroll
-          for (int i = 0; i < COLS; ++i)
-            if (i >= valid) s[i] = 0xff800000u;  // -inf
+          for (int i = 0; i < 64; ++i)
+            if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
         }
       }
-      float mx0 = max3(__uint_as_float(s[0]), __uint_as_float(s[1]), __uint_as_float(s[2]));
-      float mx1 = max3(__uint_as_float(s[3]), __uint_as_float(s[4]), __uint_as_float(s[5]));
-      float mx2 = __uint_as_float(s[6]), mx3 = __uint_as_float(s[7]);
+      float nm[2];
 #pragma unroll
-      for (int i = 8; i < COLS; i += 8) {
-        mx0 = max3(mx0, __uint_as_float(s[i]), __uint_as_float(s[i + 1]));
-        mx1 = max3(mx1, __uint_as_float(s[i + 2]), __uint_as_float(s[i + 3]));
-        mx2 = max3(mx2, __uint_as_float(s[i + 4]), __uint_as_float(s[i + 5]));
-        mx3 = max3(mx3, __uint_as_float(s[i + 6]), __uint_as_float(s[i + 7]));
-      }
-      float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-      if constexpr (kSplit == 2) {
-        // combine the two half-row maxima (both threads must take the same rescale decision)
-        float* xb = xbuf + ((t * 2 + (j & 1)) * 2) * 128;
-        xb[half * 128 + row] = mx;
-        asm volatile("bar.sync %0, 256;" ::"r"(1 + t) : "memory");
-        mx = fmaxf(mx, xb[(half ^ 1) * 128 + row]);
-      }
-      // lazy rescale: move the reference only if the max grew by more than 8 (log2 domain)
-      float alpha = 1.f;
-      const bool need = (mx - m_used) * sl2 > 8.f;  // (-inf reference => true)
-      if (need) {
-        alpha = ex2_approx((m_used - mx) * sl2);  // exp2(-inf) = 0 on the first block
-        m_used = mx;
-        l *= alpha;
-      }
-      if (j > 0 && __any_sync(0xffffffffu, need)) {
-        mbar_wait(&pv_done[t], (j - 1) & 1);  // O_t must be quiescent
-        tc_fence_after();
-        uint32_t o[32];
+      for (int hh = 0; hh < 2; ++hh) {
+        float mx = fmaxf(s[2 * hh], s[2 * hh + 1]);
 #pragma unroll
-        for (int c = 0; c < OCOLS / 32; ++c) {
-          tmem_ld32(tm_o + 32 * c, o);
-          tmem_ld_wait();
+        for (int jn = 1; jn < 16; ++jn) mx = fmaxf(mx, fmaxf(s[4 * jn + 2 * hh], s[4 * jn + 2 * hh + 1]));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        // lazy rescale: move the reference only if the max grew by more than 8 (log2 domain)
+        if ((mx - m_used[hh]) * sl2 > 8.f) {  // (-inf reference => true)
+          const float alpha = ex2_approx((m_used[hh] - mx) * sl2);  // exp2(-inf) = 0 on the first block
+          m_used[hh] = mx;
+          l[hh] *= alpha;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st32(tm_o + 32 * c, o);
+          for (int jn = 0; jn < 8; ++jn) { o[4 * jn + 2 * hh] *= alpha; o[4 * jn + 2 * hh + 1] *= alpha; }
         }
-        tmem_st_wait();
+        nm[hh] = -m_used[hh] * sl2;
       }
-      const float nm = -m_used * sl2;
-      float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-      uint32_t pk[COLS / 2];
+      // P = exp2(S sl2 - m sl2), packed to bf16 A fragments: k-step kk covers key columns [16 kk, 16 kk + 16)
+      uint32_t pa[8][4];
 #pragma unroll
-      for (int i = 0; i < COLS; i += 4) {
-        float x0, x1, x2, x3;
-        ffma2(x0, x1, __uint_as_float(s[i]), __uint_as_float(s[i + 1]), sl2, nm);
-        ffma2(x2, x3, __uint_as_float(s[i + 2]), __uint_as_float(s[i + 3]), sl2, nm);
-        float e0, e1, e2, e3;
-        if ((kMask >> ((i / 2) & 7)) & 1) exp2_emu2(e0, e1, x0, x1);
-        else { e0 = ex2_approx(x0); e1 = ex2_approx(x1); }
-        if ((kMask >> ((i / 2 + 1) & 7)) & 1) exp2_emu2(e2, e3, x2, x3);
-        else { e2 = ex2_approx(x2); e3 = ex2_approx(x3); }
-        fadd2(l0, l1, e0, e1);
-        fadd2(l2, l3, e2, e3);
-        pk[i / 2] = pack_bf16(e0, e1);
-        pk[i / 2 + 1] = pack_bf16(e2, e3);
-      }
-      l += (l0 + l1) + (l2 + l3);
-      if (j > 0) {
-        mbar_wait(&pv_done[t], (j - 1) & 1);  // previous PV has consumed P_t
-        tc_fence_after();
-      }
+      for (int kk = 0; kk < 8; ++kk) {
 #pragma unroll
-      for (int c = 0; c < COLS / 64; ++c) tmem_st32(tm_p + 32 * c, pk + 32 * c);
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(&p_full[t]);
+        for (int r = 0; r < 4; ++r) {
+          const int i = 8 * kk + 2 * r, hh = r & 1;
+          const float e0 = ex2_approx(fmaf(s[i], sl2, nm[hh])), e1 = ex2_approx(fmaf(s[i + 1], sl2, nm[hh]));
+          l[hh] += e0 + e1;
+          pa[kk][r] = pack_bf16(e0, e1);
+        }
+      }
+      mbar_wait(&v_full[st], ph);
+      {
+        const uint64_t vd = make_smem_desc_sw128(smem_u32(smem_v + st * ATT_TILE_BYTES));
+        fence_regs(o);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk)  // 16 keys per MMA: 16 smem rows (2048 B) of V
+          wgmma_rs_n64<1>(o, pa[kk], vd + 128 * kk, 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o);
+      }
+      if (wg_tid == 0) mbar_arrive(&v_empty[st]);
     }
 
-    // ---- epilogue: O / l -> bf16 -> global
-    if constexpr (kSplit == 2) {
-      float* xb = xbuf + ((t * 2 + (nkv & 1)) * 2) * 128;  // slot not used by the last iteration's exchange
-      xb[half * 128 + row] = l;
-      asm volatile("bar.sync %0, 256;" ::"r"(1 + t) : "memory");
-      l += xb[(half ^ 1) * 128 + row];
+    // ---- epilogue: O / l -> global
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
     }
-    mbar_wait(&pv_done[t], (nkv - 1) & 1);
-    tc_fence_after();
-    const int q = qt * 256 + t * 128 + row;
-    const float inv = 1.f / l;
-    if (p.part_o != nullptr) {
-      // partial result of this key slice: normalised fp32 O and its log-sum-exp; f3r_attention_merge combines slices
-      const size_t slot = static_cast<size_t>(p.part_base + split);
-      float* dstf = p.part_o + (slot * p.batch * p.sq + static_cast<size_t>(b) * p.sq + q) * dmodel + h * 64 + half * OCOLS;
 #pragma unroll
-      for (int c = 0; c < OCOLS / 32; ++c) {
-        uint32_t o[32];
-        tmem_ld32(tm_o + 32 * c, o);
-        tmem_ld_wait();
-        if (q < p.sq) {
+    for (int hh = 0; hh < 2; ++hh) {
+      const int q = qt * 128 + rw + 8 * hh;
+      if (q >= p.sq) continue;
+      const float inv = 1.f / l[hh];
+      const float lse = m_used[hh] * sl2 * 0.69314718056f + logf(l[hh]);
+      if (p.part_o != nullptr) {
+        // partial result of this key slice: normalised fp32 O and its log-sum-exp; f3r_attention_merge combines slices
+        const size_t slot = static_cast<size_t>(p.part_base + split);
+        float* dstf = p.part_o + (slot * p.batch * p.sq + static_cast<size_t>(b) * p.sq + q) * dmodel + h * 64 + cq;
 #pragma unroll
-          for (int i = 0; i < 8; ++i)
-            reinterpret_cast<float4*>(dstf + 32 * c)[i] =
-                make_float4(__uint_as_float(o[4 * i]) * inv, __uint_as_float(o[4 * i + 1]) * inv,
-                            __uint_as_float(o[4 * i + 2]) * inv, __uint_as_float(o[4 * i + 3]) * inv);
-        }
-      }
-      if (q < p.sq && half == 0)
-        p.part_lse[(slot * p.batch * p.heads + static_cast<size_t>(b) * p.heads + h) * p.sq + q] =
-            m_used * sl2 * 0.69314718056f + logf(l);
-    } else {
-    __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.out) + (static_cast<size_t>(b) * p.sq + q) * p.ldo + h * 64 +
-                         half * OCOLS;
+        for (int jn = 0; jn < 8; ++jn)
+          *reinterpret_cast<float2*>(dstf + 8 * jn) = make_float2(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv);
+        if ((lane & 3) == 0) p.part_lse[(slot * p.batch * p.heads + static_cast<size_t>(b) * p.heads + h) * p.sq + q] = lse;
+      } else {
+        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.out) + (static_cast<size_t>(b) * p.sq + q) * p.ldo + h * 64 + cq;
 #pragma unroll
-    for (int c = 0; c < OCOLS / 32; ++c) {
-      uint32_t o[32];
-      tmem_ld32(tm_o + 32 * c, o);
-      tmem_ld_wait();
-      if (q < p.sq) {
-        uint4* d4 = reinterpret_cast<uint4*>(dst + 32 * c);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 w;
-          w.x = pack_bf16(__uint_as_float(o[8 * i + 0]) * inv, __uint_as_float(o[8 * i + 1]) * inv);
-          w.y = pack_bf16(__uint_as_float(o[8 * i + 2]) * inv, __uint_as_float(o[8 * i + 3]) * inv);
-          w.z = pack_bf16(__uint_as_float(o[8 * i + 4]) * inv, __uint_as_float(o[8 * i + 5]) * inv);
-          w.w = pack_bf16(__uint_as_float(o[8 * i + 6]) * inv, __uint_as_float(o[8 * i + 7]) * inv);
-          d4[i] = w;
-        }
+        for (int jn = 0; jn < 8; ++jn)
+          *reinterpret_cast<uint32_t*>(dst + 8 * jn) = pack_bf16(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv);
+        if (p.lse != nullptr && (lane & 3) == 0) p.lse[(static_cast<size_t>(b) * p.heads + h) * p.sq + q] = lse;
       }
     }
-    if (p.lse != nullptr && q < p.sq && half == 0)
-      p.lse[(static_cast<size_t>(b) * p.heads + h) * p.sq + q] = m_used * sl2 * 0.69314718056f + logf(l);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
-template <int kEmu, int kSplit>
-static cudaError_t launch_attention_t(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a,
-                                      cudaStream_t stream) {
+cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, cudaStream_t stream) {
   // (set on every launch: the attribute is per device and one process may drive several GPUs)
-  cudaError_t e = cudaFuncSetAttribute(attention_kernel<kEmu, kSplit>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       ATT_SMEM_BYTES);
+  cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM_BYTES);
   if (e != cudaSuccess) return e;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(a.batch * a.heads * a.q_tiles * a.n_split);
-  cfg.blockDim = dim3(att_threads<kSplit>());
+  cfg.blockDim = dim3(ATT_THREADS);
   cfg.dynamicSmemBytes = ATT_SMEM_BYTES;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   cfg.attrs = attr;
   cfg.numAttrs = launch_attrs(attr, 1);
-  return cudaLaunchKernelEx(&cfg, attention_kernel<kEmu, kSplit>, tq, tkv, a);
-}
-
-#ifndef F3R_ATT_EMU_DEFAULT
-#define F3R_ATT_EMU_DEFAULT 1
-#endif
-#ifndef F3R_ATT_SPLIT_DEFAULT
-#define F3R_ATT_SPLIT_DEFAULT 2
-#endif
-
-int g_attn_emu = -1;    // f3r_set_option("attn_emu", v)
-int g_attn_split = -1;  // f3r_set_option("attn_split", v)
-
-cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, cudaStream_t stream) {
-  // kEmu of every 8 exponential pairs on the FMA pipe, kSplit softmax threads per row; F3R_ATTN_EMU / F3R_ATTN_SPLIT
-  // (or f3r_set_option) override the defaults for A/B measurements
-  if (g_attn_emu < 0) {
-    const char* e = getenv("F3R_ATTN_EMU");
-    g_attn_emu = (e && e[0] >= '0' && e[0] <= '3') ? (e[0] - '0') : F3R_ATT_EMU_DEFAULT;
-  }
-  if (g_attn_split < 0) {
-    const char* e = getenv("F3R_ATTN_SPLIT");
-    g_attn_split = (e && (e[0] == '1' || e[0] == '2')) ? (e[0] - '0') : F3R_ATT_SPLIT_DEFAULT;
-  }
-#define F3R_ATT_CASE(E)                                                                       \
-  case E: return g_attn_split == 2 ? launch_attention_t<E, 2>(tq, tkv, a, stream)             \
-                                   : launch_attention_t<E, 1>(tq, tkv, a, stream);
-  switch (g_attn_emu) {
-    F3R_ATT_CASE(1) F3R_ATT_CASE(2) F3R_ATT_CASE(3)
-    default: return g_attn_split == 2 ? launch_attention_t<0, 2>(tq, tkv, a, stream)
-                                      : launch_attention_t<0, 1>(tq, tkv, a, stream);
-  }
-#undef F3R_ATT_CASE
+  return cudaLaunchKernelEx(&cfg, attention_kernel, tq, tkv, a);
 }
 
 // ---------------------------------------------------------------- merge of key-slice partials

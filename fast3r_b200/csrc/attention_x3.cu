@@ -3,25 +3,24 @@
 //  fast3r/dust3r/inference_multiview.py:41-49 dtype="32".)
 //
 // Every fp32 operand x is carried as a pair of bf16 numbers x = hi + lo (hi = bf16(x), lo = bf16(x - hi), 16 mantissa
-// bits together) and every product is evaluated as hi*hi + lo*hi + hi*lo in the fp32 TMEM accumulator (the lo*lo term,
+// bits together) and every product is evaluated as hi*hi + lo*hi + hi*lo in the fp32 accumulator (the lo*lo term,
 // 2^-18 relative, is dropped):
 //   S = Q K^T : the head dimension is "concatenated" to 192: Q' = [Qhi | Qlo | Qhi], K' = [Khi | Khi | Klo]
 //               (written by attn_split_kernel below) -> 12 k-steps of one 128x128x16 SS MMA chain instead of 4;
-//   O += P V  : P is split in the softmax registers into Phi / Plo (two packed-bf16 TMEM operands), V arrives as
-//               [Vhi | Vlo]; three TS MMA chains Phi*Vhi + Plo*Vhi + Phi*Vlo accumulate into the same O columns.
+//   O += P V  : P is split in the softmax registers into Phi / Plo (two packed-bf16 register A operands), V arrives
+//               as [Vhi | Vlo]; three wgmma chains Phi*Vhi + Plo*Vhi + Phi*Vlo accumulate into the same O registers.
 // Softmax statistics, the row sum (of the un-split fp32 p) and the output are fp32.  One CTA = 128 query rows of one
-// (batch, head); K'/V' blocks of 128 keys stream through a 2-stage TMA ring.  This kernel trades speed for accuracy
-// (3x the MMAs, no query-tile ping-pong); the bf16 kernel in attention.cu is the fast path.
+// (batch, head), 64 per consumer warpgroup; K'/V' blocks of 128 keys stream through a 2-stage TMA ring.  This kernel
+// trades speed for accuracy (3x the MMAs); the bf16 kernel in attention.cu is the fast path.
 #include "common.cuh"
 #include "f3r_kernels.h"
 
 namespace f3r {
 
-constexpr int X3_THREADS = 256;  // warp 0 TMA, warp 1 MMA (+ TMEM alloc), warps 2-3 idle, warps 4-7 softmax
+constexpr int X3_THREADS = 384;  // warpgroup 0: TMA producer; warpgroups 1, 2: 64 query rows each
 constexpr int X3_STAGES = 2;
 constexpr int X3_TILE = 128 * 64 * 2;  // 16 KB: 128 rows x 64 bf16, 128B-swizzled
 constexpr int X3_SMEM_BYTES = (3 + X3_STAGES * 5) * X3_TILE + 1024 + 256;
-constexpr uint32_t X3_TM_S = 0, X3_TM_PHI = 128, X3_TM_PLO = 192, X3_TM_O = 256;
 
 __global__ void __launch_bounds__(X3_THREADS, 1)
 attention_x3_kernel(const __grid_constant__ CUtensorMap tmap_q3, const __grid_constant__ CUtensorMap tmap_k3,
@@ -37,11 +36,6 @@ attention_x3_kernel(const __grid_constant__ CUtensorMap tmap_q3, const __grid_co
   uint64_t* k_empty = k_full + X3_STAGES;
   uint64_t* v_full = k_empty + X3_STAGES;
   uint64_t* v_empty = v_full + X3_STAGES;
-  uint64_t* s_full = v_empty + X3_STAGES;
-  uint64_t* s_free = s_full + 1;
-  uint64_t* p_full = s_free + 1;
-  uint64_t* pv_done = p_full + 1;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(pv_done + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -57,191 +51,131 @@ attention_x3_kernel(const __grid_constant__ CUtensorMap tmap_q3, const __grid_co
     tma_prefetch_desc(&tmap_v2);
     mbar_init(q_full, 1);
     for (int s = 0; s < X3_STAGES; ++s) {
-      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1);
-      mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 1);
+      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 2);
+      mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 2);
     }
-    mbar_init(s_full, 1); mbar_init(s_free, 128); mbar_init(p_full, 128); mbar_init(pv_done, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0 && lane == 0) {
       // ===================== TMA producer =====================
       mbar_arrive_expect_tx(q_full, 3 * X3_TILE);
       for (int s = 0; s < 3; ++s) tma_load_3d(smem_q + s * X3_TILE, &tmap_q3, q_full, h * 192 + s * 64, qt * 128, b);
       int stage = 0; uint32_t phase = 0;
       for (int j = 0; j < nkv; ++j) {
-        mbar_wait(&k_empty[stage], phase ^ 1);
+        mbar_wait_relaxed(&k_empty[stage], phase ^ 1);
         mbar_arrive_expect_tx(&k_full[stage], 3 * X3_TILE);
         for (int s = 0; s < 3; ++s)
           tma_load_3d(smem_k + (stage * 3 + s) * X3_TILE, &tmap_k3, &k_full[stage], h * 192 + s * 64, j * 128, b);
-        mbar_wait(&v_empty[stage], phase ^ 1);
+        mbar_wait_relaxed(&v_empty[stage], phase ^ 1);
         mbar_arrive_expect_tx(&v_full[stage], 2 * X3_TILE);
         for (int s = 0; s < 2; ++s)
           tma_load_3d(smem_v + (stage * 2 + s) * X3_TILE, &tmap_v2, &v_full[stage], h * 128 + s * 64, j * 128, b);
         if (++stage == X3_STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===================== MMA issuer =====================
-      constexpr uint32_t idesc_qk = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, 0, 1);
-      auto issue_s = [&](int stage) {
-#pragma unroll
-        for (int s = 0; s < 3; ++s) {
-          const uint64_t qd = make_smem_desc_sw128(smem_u32(smem_q + s * X3_TILE), 1);
-          const uint64_t kd = make_smem_desc_sw128(smem_u32(smem_k + (stage * 3 + s) * X3_TILE), 1);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_ss(tmem_base + X3_TM_S, qd + 2 * k, kd + 2 * k, idesc_qk, (s | k) ? 1u : 0u);
-        }
-        umma_commit(s_full);
-        umma_commit(&k_empty[stage]);
-      };
-      auto issue_pv = [&](int stage, int j) {
-        const uint64_t vhi = make_smem_desc_sw128(smem_u32(smem_v + (stage * 2 + 0) * X3_TILE), 0);
-        const uint64_t vlo = make_smem_desc_sw128(smem_u32(smem_v + (stage * 2 + 1) * X3_TILE), 0);
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_ts(tmem_base + X3_TM_O, tmem_base + X3_TM_PHI + 8 * k, vhi + 128 * k, idesc_pv, (j > 0 || k > 0) ? 1u : 0u);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) umma_ts(tmem_base + X3_TM_O, tmem_base + X3_TM_PLO + 8 * k, vhi + 128 * k, idesc_pv, 1u);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) umma_ts(tmem_base + X3_TM_O, tmem_base + X3_TM_PHI + 8 * k, vlo + 128 * k, idesc_pv, 1u);
-        umma_commit(pv_done);
-        umma_commit(&v_empty[stage]);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      issue_s(0);
-      for (int j = 0; j < nkv; ++j) {
-        const int st = j % X3_STAGES;
-        const uint32_t ph = (j / X3_STAGES) & 1;
-        if (j + 1 < nkv) {
-          const int st1 = (j + 1) % X3_STAGES;
-          const uint32_t ph1 = ((j + 1) / X3_STAGES) & 1;
-          mbar_wait(&k_full[st1], ph1);
-          mbar_wait(s_free, j & 1);  // the softmax warps hold S_j in registers
-          tc_fence_after();
-          issue_s(st1);
-        }
-        mbar_wait(&v_full[st], ph);
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
-        issue_pv(st, j);
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== softmax warps: one thread per query row =====================
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(quarter * 32) << 16;
-    const uint32_t tm_s = tmem_base + lane_base + X3_TM_S;
-    const uint32_t tm_phi = tmem_base + lane_base + X3_TM_PHI;
-    const uint32_t tm_plo = tmem_base + lane_base + X3_TM_PLO;
-    const uint32_t tm_o = tmem_base + lane_base + X3_TM_O;
+  } else {
+    // ===================== consumer warpgroups (fragment layout: see common.cuh) =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cg = (warp - 4) >> 2;
+    const int wg_tid = threadIdx.x & 127;
+    const int rw = cg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
     const float sl2 = p.scale_log2;
-    float m_used = -INFINITY, l = 0.f;
-    for (int j = 0; j < nkv; ++j) {
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      uint32_t s[128];
+    float m_used[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    float o[32];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) tmem_ld32(tm_s + 32 * c, s + 32 * c);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(s_free);
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < nkv; ++j) {
+      const int st = j % X3_STAGES;
+      const uint32_t ph = (j / X3_STAGES) & 1;
+      float s[64];
+      mbar_wait(&k_full[st], ph);
+      wgmma_fence();
+#pragma unroll
+      for (int t = 0; t < 3; ++t) {
+        const uint64_t qd = make_smem_desc_sw128(smem_u32(smem_q + t * X3_TILE + cg * 64 * 128));
+        const uint64_t kd = make_smem_desc_sw128(smem_u32(smem_k + (st * 3 + t) * X3_TILE));
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_ss_n128<0>(s, qd + 2 * k, kd + 2 * k, (t | k) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      if (wg_tid == 0) mbar_arrive(&k_empty[st]);
       if (j == nkv - 1) {
         const int valid = p.skv - j * 128;
         if (valid < 128) {
 #pragma unroll
-          for (int i = 0; i < 128; ++i)
-            if (i >= valid) s[i] = 0xff800000u;  // -inf
+          for (int i = 0; i < 64; ++i)
+            if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
         }
       }
-      float mx = __uint_as_float(s[0]);
+      float nm[2];
 #pragma unroll
-      for (int i = 1; i < 128; ++i) mx = fmaxf(mx, __uint_as_float(s[i]));
-      float alpha = 1.f;
-      const bool need = (mx - m_used) * sl2 > 8.f;  // lazy reference move (first block: -inf reference => true)
-      if (need) {
-        alpha = exp2f((m_used - mx) * sl2);
-        m_used = mx;
-        l *= alpha;
-      }
-      if (j > 0) {
-        mbar_wait(pv_done, (j - 1) & 1);  // O quiescent, P_{j-1} consumed
-        tc_fence_after();
-        if (__any_sync(0xffffffffu, need)) {
-          uint32_t o[32];
+      for (int hh = 0; hh < 2; ++hh) {
+        float mx = fmaxf(s[2 * hh], s[2 * hh + 1]);
 #pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            tmem_ld32(tm_o + 32 * c, o);
-            tmem_ld_wait();
+        for (int jn = 1; jn < 16; ++jn) mx = fmaxf(mx, fmaxf(s[4 * jn + 2 * hh], s[4 * jn + 2 * hh + 1]));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        if ((mx - m_used[hh]) * sl2 > 8.f) {  // lazy reference move (first block: -inf reference => true)
+          const float alpha = exp2f((m_used[hh] - mx) * sl2);
+          m_used[hh] = mx;
+          l[hh] *= alpha;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st32(tm_o + 32 * c, o);
-          }
-          tmem_st_wait();
+          for (int jn = 0; jn < 8; ++jn) { o[4 * jn + 2 * hh] *= alpha; o[4 * jn + 2 * hh + 1] *= alpha; }
         }
+        nm[hh] = -m_used[hh] * sl2;
       }
-      const float nm = -m_used * sl2;
-      float lsum = 0.f;
+      uint32_t phi[8][4], plo[8][4];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t hi[16], lo[16];
+      for (int kk = 0; kk < 8; ++kk) {
 #pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const float e0 = exp2f(fmaf(__uint_as_float(s[32 * c + i]), sl2, nm));
-          const float e1 = exp2f(fmaf(__uint_as_float(s[32 * c + i + 1]), sl2, nm));
-          lsum += e0 + e1;
+        for (int r = 0; r < 4; ++r) {
+          const int i = 8 * kk + 2 * r, hh = r & 1;
+          const float e0 = exp2f(fmaf(s[i], sl2, nm[hh])), e1 = exp2f(fmaf(s[i + 1], sl2, nm[hh]));
+          l[hh] += e0 + e1;
           const uint32_t h2 = pack_bf16(e0, e1);
-          hi[i / 2] = h2;
-          lo[i / 2] = pack_bf16(e0 - bf16_lo(h2), e1 - bf16_hi(h2));
+          phi[kk][r] = h2;
+          plo[kk][r] = pack_bf16(e0 - bf16_lo(h2), e1 - bf16_hi(h2));
         }
-        tmem_st16(tm_phi + 16 * c, hi);
-        tmem_st16(tm_plo + 16 * c, lo);
       }
-      l += lsum;
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(p_full);
+      mbar_wait(&v_full[st], ph);
+      const uint64_t vhi = make_smem_desc_sw128(smem_u32(smem_v + (st * 2 + 0) * X3_TILE));
+      const uint64_t vlo = make_smem_desc_sw128(smem_u32(smem_v + (st * 2 + 1) * X3_TILE));
+      fence_regs(o);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) wgmma_rs_n64<1>(o, phi[kk], vhi + 128 * kk, 1u);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) wgmma_rs_n64<1>(o, plo[kk], vhi + 128 * kk, 1u);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) wgmma_rs_n64<1>(o, phi[kk], vlo + 128 * kk, 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(o);
+      if (wg_tid == 0) mbar_arrive(&v_empty[st]);
     }
     // ---- epilogue: O / l -> fp32 global
-    mbar_wait(pv_done, (nkv - 1) & 1);
-    tc_fence_after();
-    const int q = qt * 128 + row;
-    const float inv = 1.f / l;
-    float* dst = static_cast<float*>(p.out) + (static_cast<size_t>(b) * p.sq + q) * p.ldo + h * 64;
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint32_t o[32];
-      tmem_ld32(tm_o + 32 * c, o);
-      tmem_ld_wait();
-      if (q < p.sq) {
+    for (int hh = 0; hh < 2; ++hh) {
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
+      l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 2);
+      const int q = qt * 128 + rw + 8 * hh;
+      if (q >= p.sq) continue;
+      const float inv = 1.f / l[hh];
+      float* dst = static_cast<float*>(p.out) + (static_cast<size_t>(b) * p.sq + q) * p.ldo + h * 64 + cq;
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-          reinterpret_cast<float4*>(dst + 32 * c)[i] =
-              make_float4(__uint_as_float(o[4 * i]) * inv, __uint_as_float(o[4 * i + 1]) * inv,
-                          __uint_as_float(o[4 * i + 2]) * inv, __uint_as_float(o[4 * i + 3]) * inv);
-      }
+      for (int jn = 0; jn < 8; ++jn)
+        *reinterpret_cast<float2*>(dst + 8 * jn) = make_float2(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv);
+      if (p.lse != nullptr && (lane & 3) == 0)
+        p.lse[(static_cast<size_t>(b) * p.heads + h) * p.sq + q] = m_used[hh] * sl2 * 0.69314718056f + logf(l[hh]);
     }
-    if (p.lse != nullptr && q < p.sq)
-      p.lse[(static_cast<size_t>(b) * p.heads + h) * p.sq + q] = m_used * sl2 * 0.69314718056f + logf(l);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
@@ -293,7 +227,7 @@ cudaError_t launch_attn_split(const float* q, int ldq, const float* kv, int ldkv
   if (ldq % 4 || ldkv % 4) return cudaErrorInvalidValue;
   const size_t total = (rows_q + 2 * rows_kv) * heads * 16;
   if (total == 0) return cudaSuccess;
-  const int grid = static_cast<int>(total / 256 + 1 < 148 * 16 ? total / 256 + 1 : 148 * 16);
+  const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
   attn_split_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4*>(q), ldq / 4,
                                               reinterpret_cast<const float4*>(kv), ldkv / 4, static_cast<uint2*>(q3),
                                               static_cast<uint2*>(k3), static_cast<uint2*>(v2), rows_q, rows_kv, heads);
@@ -321,7 +255,7 @@ cudaError_t launch_split3(const float* in, void* out, size_t rows, int k, int re
   if (k % 4) return cudaErrorInvalidValue;
   const size_t total = rows * (k / 4);
   if (total == 0) return cudaSuccess;
-  const int grid = static_cast<int>(total / 256 + 1 < 148 * 16 ? total / 256 + 1 : 148 * 16);
+  const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
   split3_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4*>(in), static_cast<uint2*>(out), rows, k / 4, relu);
   return cudaGetLastError();
 }
@@ -340,7 +274,7 @@ cudaError_t launch_add_f32(float* dst, const float* src, size_t n, cudaStream_t 
   if (n % 4) return cudaErrorInvalidValue;
   if (n == 0) return cudaSuccess;
   const size_t n4 = n / 4;
-  const int grid = static_cast<int>(n4 / 256 + 1 < 148 * 16 ? n4 / 256 + 1 : 148 * 16);
+  const int grid = static_cast<int>(n4 / 256 + 1 < 132 * 16 ? n4 / 256 + 1 : 132 * 16);
   add_f32_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<float4*>(dst), reinterpret_cast<const float4*>(src), n4);
   return cudaGetLastError();
 }

@@ -66,10 +66,10 @@ int make_tmap(CUtensorMap* m, const void* ptr, int rank, const uint64_t* dims, c
 int num_sms() {
   static int cache[64] = {0};  // per device: one process may drive several GPUs
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   int& n = cache[dev & 63];
   if (n) return n;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   return n;
 }
 
@@ -84,19 +84,9 @@ uint64_t f3r_launch_count(void) { return g_launches.load(); }
 
 int f3r_set_option(const char* name, int32_t value) {
   if (!name) return fail("f3r_set_option: null name");
-  if (!strcmp(name, "attn_emu")) {
-    if (value < -1 || value > 3) return fail("f3r_set_option: attn_emu must be in [-1, 3]");
-    f3r::g_attn_emu = value;
-    return 0;
-  }
   if (!strcmp(name, "pdl")) {
     if (value != 0 && value != 1) return fail("f3r_set_option: pdl must be 0 or 1");
     f3r::g_pdl = value;
-    return 0;
-  }
-  if (!strcmp(name, "attn_split")) {
-    if (value != -1 && value != 1 && value != 2) return fail("f3r_set_option: attn_split must be -1, 1 or 2");
-    f3r::g_attn_split = value;
     return 0;
   }
   return fail("f3r_set_option: unknown option '%s'", name);
@@ -139,13 +129,6 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
     if (tiles256 >= num_sms()) block_n = 256;
   }
   a.num_n_tiles = (d->n + block_n - 1) / block_n;
-  // CTA pairs sharing the weight tile through TMA multicast (F3R_GEMM_CLUSTER=1 disables, for A/B measurements)
-  static int cluster_pref = -1;
-  if (cluster_pref < 0) {
-    const char* e = getenv("F3R_GEMM_CLUSTER");
-    cluster_pref = (e && e[0] == '1') ? 1 : 2;
-  }
-  const int cluster = (cluster_pref == 2 && a.num_m_tiles >= 2) ? 2 : 1;
   static int dbg = -1, tma_pref = -1;
   if (dbg < 0) { const char* e = getenv("F3R_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }
   if (tma_pref < 0) { const char* e = getenv("F3R_GEMM_TMA_EPI"); tma_pref = (e && e[0] == '0') ? 0 : 1; }
@@ -175,7 +158,7 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
     const uint64_t dims[3] = {static_cast<uint64_t>(d->k), static_cast<uint64_t>(d->taps),
                               static_cast<uint64_t>(d->n)};
     const uint64_t str[2] = {static_cast<uint64_t>(d->k) * 2, static_cast<uint64_t>(d->k) * 2 * d->taps};
-    const uint32_t box[3] = {64, 1, static_cast<uint32_t>(block_n / cluster)};
+    const uint32_t box[3] = {64, 1, static_cast<uint32_t>(block_n)};
     if (make_tmap(&tb, d->wt, 3, dims, str, box)) return 1;
   }
   // TMA epilogue for the hot cases: plain (activated) stores, and the in-place fp32 residual update as a reduce-add
@@ -212,9 +195,9 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
   static int ksplit_pref = -1;  // F3R_GEMM_KSPLIT=1 disables the K slicing (A/B measurements)
   if (ksplit_pref < 0) { const char* e = getenv("F3R_GEMM_KSPLIT"); ksplit_pref = (e && e[0] == '1') ? 1 : 0; }
   if (a.tma_epi == 2 && d->taps == 1 && ksplit_pref != 1) {
-    // x += A W^T with fewer output tiles than SM (pairs): cut K into slices, each CTA reduce-adds its partial sum
-    const long slots = num_sms() / cluster;
-    const long items = static_cast<long>((a.num_m_tiles + cluster - 1) / cluster) * a.num_n_tiles;
+    // x += A W^T with fewer output tiles than SMs: cut K into slices, each CTA reduce-adds its partial sum
+    const long slots = num_sms();
+    const long items = static_cast<long>(a.num_m_tiles) * a.num_n_tiles;
     const int k_iters = (d->k + 63) / 64;
     double best = 1e30;
     for (int s = 1; s <= 4 && (s == 1 || k_iters / s >= 16); ++s) {  // (short K: the reduce-add epilogue dominates, slicing loses)
@@ -223,7 +206,7 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
     }
   }
   g_launches++;
-  return check(f3r::launch_gemm(block_n, cluster, ta, tb, to0, to0b, a, num_sms(), static_cast<cudaStream_t>(stream)),
+  return check(f3r::launch_gemm(block_n, ta, tb, to0, to0b, a, num_sms(), static_cast<cudaStream_t>(stream)),
                "f3r_gemm");
 }
 
@@ -254,7 +237,7 @@ static int attention_impl(const char* what, const void* q, int32_t ldq, const vo
   f3r::AttnArgs a;
   memset(&a, 0, sizeof(a));
   a.batch = batch; a.heads = heads; a.sq = sq; a.skv = skv;
-  a.q_tiles = (sq + 255) / 256;
+  a.q_tiles = (sq + 127) / 128;
   a.scale_log2 = scale * 1.4426950408889634f;
   a.ldo = ldo; a.out = out; a.lse = lse;
   a.kv_row0 = kv_row0; a.n_split = n_split; a.part_base = part_base; a.part_o = part_o; a.part_lse = part_lse;

@@ -1,7 +1,6 @@
-// Blackwell (sm_100a) PTX wrappers shared by the fast3r_b200 kernels: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st / fences), UMMA descriptors.
-// Hand-written inline PTX; descriptor bit layouts follow the PTX ISA tcgen05 "matrix descriptor"
-// and "instruction descriptor" tables.
+// Hopper (sm_90a) PTX wrappers shared by the fast3r_b200 kernels: mbarrier, TMA (cp.async.bulk.tensor),
+// warpgroup MMA (wgmma.mma_async) and its shared-memory matrix descriptors.  Hand-written inline PTX; the descriptor
+// bit layout follows the PTX ISA "matrix descriptor format" table for wgmma.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -86,17 +85,6 @@ F3R_DEVICE void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int 
       : "memory");
 }
 
-F3R_DEVICE void tma_load_3d_mcast(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                  uint16_t cta_mask) {
-  // the box lands at the same smem offset, and completes on the mbarrier at the same offset, in every CTA of cta_mask
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4, %5}], [%2], %6;"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
-      "h"(cta_mask)
-      : "memory");
-}
-
 // ------------------------------------------------------------------ TMA stores (smem -> global, bulk_group completion)
 F3R_DEVICE void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
@@ -115,7 +103,7 @@ F3R_DEVICE void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;
 
 // ------------------------------------------------------------------ programmatic dependent launch
 // Kernels of the hot chain are launched with cudaLaunchAttributeProgrammaticStreamSerialization (f3r::pdl_enabled()): the
-// next kernel's CTAs may become resident, run their prologue (barrier init, TMEM allocation, descriptor prefetch) and park
+// next kernel's CTAs may become resident, run their prologue (barrier init, descriptor prefetch) and park
 // at pdl_wait() while the previous kernel drains its last wave.  pdl_wait() returns when ALL memory operations of the
 // preceding grid are complete and visible, so every access to global memory must come after it; pdl_launch_dependents()
 // only allows the successor to be scheduled early.  Without the launch attribute both are no-ops.
@@ -131,105 +119,67 @@ F3R_DEVICE void cluster_sync_all() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05: TMEM alloc
-template <uint32_t kCols>
-F3R_DEVICE void tmem_alloc(uint32_t* dst_smem) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-F3R_DEVICE void tmem_dealloc(uint32_t taddr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-F3R_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-F3R_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ------------------------------------------------------------------ tcgen05: MMA
-// Shared-memory matrix descriptor, 128-byte swizzle, rows of 128 bytes (64 bf16), 8-row groups 1024 B apart.
-//  K-major  (operand rows = M/N index, 64 contiguous K elements per row): LBO = 1 (unused), SBO = 1024 B
-//  MN-major (smem rows = K index, 64 contiguous M/N elements per row):    LBO = 0 (single 64-wide group), SBO = 1024 B
-F3R_DEVICE uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_enc) {
+// ------------------------------------------------------------------ wgmma
+// Shared-memory matrix descriptor, 128-byte swizzle, rows of 128 bytes (64 bf16), 8-row groups 1024 B apart
+// (tiles 1024-byte aligned, so the base-offset field stays 0).
+//  K-major  (operand rows = M/N index, 64 contiguous K elements per row): LBO unused (1), SBO = 1024 B;
+//           a 16-element K step inside the swizzle row is +32 B, i.e. +2 in the (addr >> 4) field.
+//  MN-major (smem rows = K index, 64 contiguous M/N elements per row):    LBO unused (1), SBO = 1024 B;
+//           a 16-element K step is 16 rows = +2048 B, i.e. +128 in the (addr >> 4) field.
+F3R_DEVICE uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);   // start address, bits [0,14)
-  d |= static_cast<uint64_t>(lbo_enc & 0x3FFF) << 16;       // leading byte offset >> 4
+  d |= static_cast<uint64_t>(1) << 16;                      // leading byte offset >> 4 (unused with 128B swizzle)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;              // stride byte offset >> 4
-  d |= static_cast<uint64_t>(1) << 46;                      // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                      // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                      // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32.
-F3R_DEVICE constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-  return (1u << 4) /*D=f32*/ | (1u << 7) /*A=bf16*/ | (1u << 10) /*B=bf16*/ | (a_mn_major << 15) |
-         (b_mn_major << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]
-F3R_DEVICE void umma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-F3R_DEVICE void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once every tcgen05 op issued so far by this thread has completed.
-F3R_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+F3R_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+F3R_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+F3R_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+// Keeps the compiler from moving accesses of accumulator registers across wgmma issue / wait points.
+template <int kN>
+F3R_DEVICE void fence_regs(float (&d)[kN]) {
+#pragma unroll
+  for (int i = 0; i < kN; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// same, arriving on the barrier at this smem offset in every CTA of cta_mask
-F3R_DEVICE void umma_commit_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
+// Accumulator fragment of an m64nN wgmma (per warpgroup): warp w of the warpgroup holds rows 16w + lane/4 (+8);
+// d[4j + 2h + e] is row 16w + lane/4 + 8h, column 8j + 2 (lane % 4) + e.
+
+// D[64 x 128] (+)= A[smem] * B[smem]^T (both K-major unless trans_b: B MN-major)
+template <int kTransB>
+F3R_DEVICE void wgmma_ss_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, %67;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(kTransB));
 }
 
-// ------------------------------------------------------------------ tcgen05: TMEM <-> registers
-// 32 lanes x 32 bit, 32 consecutive columns: thread i of the warp gets lane (base_lane + i), columns [c, c+32).
-F3R_DEVICE void tmem_ld32(uint32_t taddr, uint32_t* r) {
+// D[64 x 256] (+)= A[smem] * B[smem]^T (both K-major unless trans_b: B MN-major)
+template <int kTransB>
+F3R_DEVICE void wgmma_ss_n256(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, %131;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(kTransB));
 }
-F3R_DEVICE void tmem_st32(uint32_t taddr, const uint32_t* r) {
+
+// D[64 x 64] (+)= A[registers: 4 x packed bf16x2 per thread] * B[smem] (B MN-major if kTransB)
+template <int kTransB>
+F3R_DEVICE void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate), "n"(kTransB));
 }
-F3R_DEVICE void tmem_st16(uint32_t taddr, const uint32_t* r) {  // 16 consecutive 32-bit columns per lane
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-F3R_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-F3R_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ misc math
 F3R_DEVICE uint32_t pack_bf16(float lo, float hi) {

@@ -140,7 +140,7 @@ cudaError_t launch_im2col_patch(const float* img, void* out, int out_f32, int n,
   if (patch != 16 || H % 16 || W % 16) return cudaErrorInvalidValue;
   const size_t total = static_cast<size_t>(n) * (H / 16) * (W / 16) * 96;
   if (total == 0) return cudaSuccess;
-  const int grid = static_cast<int>(total / 256 + 1 < 148 * 16 ? total / 256 + 1 : 148 * 16);
+  const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
   if (out_f32) im2col_patch_kernel<true><<<grid, 256, 0, stream>>>(img, out, n, H, W);
   else im2col_patch_kernel<false><<<grid, 256, 0, stream>>>(img, out, n, H, W);
   return cudaGetLastError();
@@ -169,7 +169,7 @@ cudaError_t launch_im2col3x3s2(const void* in, void* out, int n, int H, int W, i
   if (C % 8) return cudaErrorInvalidValue;
   const size_t total = static_cast<size_t>(n) * Ho * Wo * 9 * (C / 8);
   if (total == 0) return cudaSuccess;
-  const int grid = static_cast<int>(total / 256 + 1 < 148 * 16 ? total / 256 + 1 : 148 * 16);
+  const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
   im2col3x3s2_kernel<<<grid, 256, 0, stream>>>(static_cast<const uint4*>(in), static_cast<uint4*>(out), n, H, W,
                                                C / 8, Ho, Wo);
   return cudaGetLastError();
@@ -289,7 +289,7 @@ cudaError_t launch_cast_bf16(const float* in, void* out, size_t n, cudaStream_t 
   if (n % 4) return cudaErrorInvalidValue;
   if (n == 0) return cudaSuccess;
   const size_t n4 = n / 4;
-  const int grid = static_cast<int>(n4 / 256 + 1 < 148 * 16 ? n4 / 256 + 1 : 148 * 16);
+  const int grid = static_cast<int>(n4 / 256 + 1 < 132 * 16 ? n4 / 256 + 1 : 132 * 16);
   cast_bf16_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4*>(in), static_cast<uint2*>(out), n4);
   return cudaGetLastError();
 }

@@ -45,12 +45,12 @@ struct GemmArgs {
   float* conf;
 };
 
-cudaError_t launch_gemm(int block_n, int cluster, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
+cudaError_t launch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
                         const CUtensorMap& to0b, const GemmArgs& a, int num_sms, cudaStream_t stream);
 
 struct AttnArgs {
   int batch, heads, sq, skv;  // per-batch query / key lengths
-  int q_tiles;                // ceil(sq / 256)
+  int q_tiles;                // ceil(sq / 128)
   float scale_log2;           // softmax scale * log2(e)
   int ldo;                    // row stride of out (elements)
   void* out;                  // bf16 [batch*sq, ldo], head h at columns h*64
@@ -67,10 +67,8 @@ struct AttnArgs {
 cudaError_t launch_attention_merge(const float* part_o, const float* part_lse, int n_parts, int batch, int heads, int sq,
                                    void* out, int ldo, cudaStream_t stream);
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, cudaStream_t stream);
-extern int g_attn_emu;    // exponential pairs (of every 8) evaluated on the FMA pipe, -1 = default
-extern int g_attn_split;  // softmax threads per query row (1 or 2), -1 = default
 
-// parity mode (attention_x3.cu): hi/lo-split bf16 operands, fp32 out (AttnArgs.out is float*, q_tiles = ceil(sq / 128))
+// parity mode (attention_x3.cu): hi/lo-split bf16 operands, fp32 out (AttnArgs.out is float*)
 cudaError_t launch_attention_x3(const CUtensorMap& tq3, const CUtensorMap& tk3, const CUtensorMap& tv2,
                                 const AttnArgs& a, cudaStream_t stream);
 cudaError_t launch_attn_split(const float* q, int ldq, const float* kv, int ldkv, void* q3, void* k3, void* v2,

@@ -1,12 +1,12 @@
-// Persistent warp-specialised tcgen05 GEMM / implicit-GEMM convolution for sm_100a.
+// Persistent warp-specialised wgmma GEMM / implicit-GEMM convolution for sm_90a.
 //
 //   out[m, n] = epilogue( sum_{tap, k} A[pixel(m) + shift(tap), k] * Wt[n, tap, k] )
 //
 // A is a channels-last bf16 activation viewed as (C, W, H, NB) and fetched by 4-D TMA boxes of
 // 128 pixels x 64 channels (out-of-bounds pixels/channels are zero-filled by TMA, which gives the
 // 3x3 zero padding and the K / N tails for free).  A plain linear layer is the 1-tap case with
-// W = rows.  Accumulation happens in TMEM (two BLOCK_N-column stages so the epilogue of tile i
-// overlaps the MMAs of tile i+1); one elected thread issues tcgen05.mma, one thread issues TMA.
+// W = rows.  One producer thread issues TMA into a multi-stage smem ring; two consumer warpgroups each
+// own 64 rows of the 128-row tile and accumulate in registers with wgmma (m64 x BLOCK_N x k16).
 //
 // Covers (reference file:line in DESIGN.md): nn.Linear qkv/proj/fc1/fc2/decoder_embed
 // (fast3r/croco/models/blocks.py:94-97,125-128; fast3r/models/fast3r.py:673), patch-embed conv as
@@ -18,19 +18,21 @@ namespace f3r {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int GEMM_THREADS = 384;  // warpgroup 0: warp0 TMA, warp1 MMA(+TMEM alloc), 2 idle; warps 4-11 epilogue
+constexpr int GEMM_THREADS = 384;  // warpgroup 0: warp 0 TMA, warps 1-3 idle; warpgroups 1, 2: wgmma + epilogue
+constexpr int XCH_STRIDE = 68;     // fp32 row stride of the fragment -> row exchange tile (64 rows x 64 columns)
 
 template <int BLOCK_N>
 struct GemmCfg {
-  static constexpr int kStages = (BLOCK_N == 256) ? 4 : 6;
+  static constexpr int kStages = (BLOCK_N == 256) ? 3 : 4;
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 1024 /*barriers*/ + 8 * 4096 /*epilogue staging*/;
-  static constexpr uint32_t kTmemCols = 2 * BLOCK_N;
+  static constexpr int kXchBytes = 64 * XCH_STRIDE * 4;  // per consumer warpgroup
+  static constexpr int kSmemBytes =
+      kStages * kStageBytes + 1024 /*align*/ + 1024 /*barriers*/ + 8 * 4096 /*epilogue staging*/ + 2 * kXchBytes;
 };
 
-// Epilogue data movement.  A thread owns one accumulator ROW (tcgen05.ld 32x32b), but row-per-thread global
+// Epilogue data movement.  A thread owns one accumulator ROW (after the fragment exchange), but row-per-thread global
 // accesses touch 32 different cache lines per instruction.  Every 32x32 fp32 chunk is therefore transposed through a
 // per-warp 4 KB shared-memory tile (16-byte chunks XOR-swizzled by row, conflict-free both ways) and all global
 // traffic (residual reads, stores) is issued in the "transposed" mapping: lane l handles 4 consecutive columns
@@ -70,43 +72,23 @@ __device__ __forceinline__ void prefetch_res(const GemmArgs& p, ResChunk& rc, si
 }
 
 // exact-erf GELU (nn.GELU(), fast3r/croco/models/blocks.py:83) with erf from Abramowitz-Stegun 7.1.26
-// (|abs err| <= 1.5e-7, far below the bf16 rounding of the stored activation), evaluated on PAIRS with the packed
-// fp32x2 FMA pipe ops (FFMA2 / FMUL2): per pair 12 packed ops + 4 MUFU (2 rcp, 2 ex2) + 2 sign merges.
-__device__ __forceinline__ void mul2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-  asm("{ .reg .b64 ra, rb, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mul.rn.f32x2 rd, ra, rb; mov.b64 {%0,%1}, rd; }"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1));
-}
-__device__ __forceinline__ void fma2(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) {
-  asm("{ .reg .b64 ra, rb, rc, rd; mov.b64 ra, {%2,%3}; mov.b64 rb, {%4,%5}; mov.b64 rc, {%6,%7};\n\t"
-      "fma.rn.f32x2 rd, ra, rb, rc; mov.b64 {%0,%1}, rd; }"
-      : "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(b0), "f"(b1), "f"(c0), "f"(c1));
-}
-__device__ __forceinline__ void gelu_fast2(float& x0, float& x1) {
-  float z0, z1;
-  mul2(z0, z1, fabsf(x0), fabsf(x1), 0.70710678118654752440f, 0.70710678118654752440f);
-  float u0, u1;
-  fma2(u0, u1, z0, z1, 0.3275911f, 0.3275911f, 1.0f, 1.0f);
-  float t0, t1;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t0) : "f"(u0));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t1) : "f"(u1));
-  float p0, p1;
-  fma2(p0, p1, t0, t1, 1.061405429f, 1.061405429f, -1.453152027f, -1.453152027f);
-  fma2(p0, p1, p0, p1, t0, t1, 1.421413741f, 1.421413741f);
-  fma2(p0, p1, p0, p1, t0, t1, -0.284496736f, -0.284496736f);
-  fma2(p0, p1, p0, p1, t0, t1, 0.254829592f, 0.254829592f);
-  mul2(p0, p1, p0, p1, t0, t1);
-  float a0, a1;
-  mul2(a0, a1, z0, z1, z0, z1);
-  mul2(a0, a1, a0, a1, -1.4426950408889634f, -1.4426950408889634f);
-  float e0, e1;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(a0));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
-  float r0, r1;                                   // erf(|z|) = 1 - poly * exp(-z^2)
-  fma2(r0, r1, p0, p1, -e0, -e1, 1.0f, 1.0f);
-  r0 = copysignf(r0, x0); r1 = copysignf(r1, x1);
-  float h0, h1;
-  mul2(h0, h1, x0, x1, 0.5f, 0.5f);
-  fma2(x0, x1, h0, h1, r0, r1, h0, h1);           // 0.5 x (1 + erf)
+// (|abs err| <= 1.5e-7, far below the bf16 rounding of the stored activation): 12 FMA-pipe ops + 2 MUFU (rcp, ex2).
+__device__ __forceinline__ void gelu_fast(float& x) {
+  const float z = __fmul_rn(fabsf(x), 0.70710678118654752440f);
+  const float u = fmaf(z, 0.3275911f, 1.0f);
+  float t;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(u));
+  float q = fmaf(t, 1.061405429f, -1.453152027f);
+  q = fmaf(q, t, 1.421413741f);
+  q = fmaf(q, t, -0.284496736f);
+  q = fmaf(q, t, 0.254829592f);
+  q = __fmul_rn(q, t);
+  const float a = __fmul_rn(__fmul_rn(z, z), -1.4426950408889634f);
+  float e;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(a));
+  const float r = copysignf(fmaf(q, -e, 1.0f), x);  // erf(|z|) = 1 - poly * exp(-z^2)
+  const float h = __fmul_rn(x, 0.5f);
+  x = fmaf(h, r, h);                                 // 0.5 x (1 + erf)
 }
 // Row-domain part: bias, RoPE, image-index embedding, or the FINAL 128->4 dot product.  Returns false if the chunk is
 // fully consumed here (FINAL).
@@ -214,7 +196,7 @@ __device__ __forceinline__ void epilogue_store(const GemmArgs& p, const float (&
     if (p.act == ACT_RELU) {
       x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f);
     } else if (p.act == ACT_GELU) {
-      gelu_fast2(x0, x1); gelu_fast2(x2, x3);
+      gelu_fast(x0); gelu_fast(x1); gelu_fast(x2); gelu_fast(x3);
     }
     void* base = p.out0;
     size_t o = off;
@@ -246,7 +228,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmArgs& p, float (&v)[32], 
     for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], 0.f);
   } else if (p.act == ACT_GELU) {
 #pragma unroll
-    for (int i = 0; i < 32; i += 2) gelu_fast2(v[i], v[i + 1]);
+    for (int i = 0; i < 32; ++i) gelu_fast(v[i]);
   }
   if (lane == 0) tma_store_wait_read();  // the previous tile of this warp has left the staging buffer
   __syncwarp();
@@ -275,10 +257,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmArgs& p, float (&v)[32], 
   }
 }
 
-// kCluster = 2: CTA pairs own vertically adjacent 128-row tiles of the same BLOCK_N column block; each CTA fetches
-// half of the shared weight tile and TMA-multicasts it to both, cutting L2->SM operand traffic per FLOP by 1/3
-// (the kernel is L2-feed bound with one CTA per tile: 48 KB per 128x256x64 k-block vs ~45-55 B/clk/SM of TMA fill).
-template <int BLOCK_N, int kCluster>
+template <int BLOCK_N>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_o0, const __grid_constant__ CUtensorMap tmap_o0b,
@@ -291,12 +270,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
-  uint64_t* tmem_full = bars + 2 * Cfg::kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   uint8_t* stage_base = smem + Cfg::kStages * Cfg::kStageBytes + 1024;  // 8 x 4 KB, 1024-aligned
-  float* fin_smem = reinterpret_cast<float*>(stage_base);  // [2][128][4] (FINAL mode does not stage)
+  float* fin_smem = reinterpret_cast<float*>(stage_base);  // [128][4] (FINAL mode does not stage)
   float* w4_smem = reinterpret_cast<float*>(stage_base + 4096);  // FINAL: [4][N <= 256] copy of the 1x1 conv weights
+  float* xch_base = reinterpret_cast<float*>(stage_base + 8 * 4096);  // [2][64][XCH_STRIDE]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -304,159 +281,144 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kCluster); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], 8); }
+    for (int s = 0; s < Cfg::kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_ptr);
   if (p.epi == EPI_FINAL)
     for (int i = threadIdx.x; i < 4 * p.N; i += GEMM_THREADS) w4_smem[i] = __ldg(p.w4 + i);
-  tc_fence_before();
   __syncthreads();
-  if constexpr (kCluster > 1) cluster_sync_all();  // peer barriers are initialised before any multicast can arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   pdl_wait();                // operands / residual are produced by the preceding kernels: no global access above this line
   pdl_launch_dependents();   // except the 1x1-conv weights of FINAL and the tensor-map prefetch (parameters, not activations)
 
-  // work item = (group of kCluster vertically adjacent m-tiles, n-tile); both CTAs of a cluster walk the same items
-  const int cta_rank = kCluster > 1 ? static_cast<int>(cluster_ctarank()) : 0;
-  const int first_item = kCluster > 1 ? static_cast<int>(cluster_id_x()) : static_cast<int>(blockIdx.x);
-  const int item_stride = kCluster > 1 ? static_cast<int>(num_clusters_x()) : static_cast<int>(gridDim.x);
   // split-K (only with the fp32 reduce-add epilogue, x += A W^T: partial sums of the K slices are added by the memory
   // system): work item = (tile, K slice); used when there are fewer tiles than SMs (small M in sequence-parallel runs)
-  const int num_out_tiles = ((p.num_m_tiles + kCluster - 1) / kCluster) * p.num_n_tiles;
+  const int num_out_tiles = p.num_m_tiles * p.num_n_tiles;
   const int num_tiles = num_out_tiles * p.k_split;
-  constexpr uint16_t kMask = (1u << kCluster) - 1;
   const int k_chunks = (p.K + BLOCK_K - 1) / BLOCK_K;
   const int k_iters = p.taps * k_chunks;
 
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");   // 384 x 168 = 128 x 72 + 256 x 216
-  if (warp == 0) {
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");   // 128 x 40 + 256 x 232 <= 64K registers
+    if (warp == 0 && lane == 0) {
       // ===================== TMA producer =====================
       int stage = 0; uint32_t phase = 0;
-      for (int item = first_item; item < num_tiles; item += item_stride) {
+      for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
         const int tile = item % num_out_tiles, ks = item / num_out_tiles;
         const int it0 = ks * k_iters / p.k_split, it1 = (ks + 1) * k_iters / p.k_split;
-        const int mt = (tile / p.num_n_tiles) * kCluster + cta_rank, nt = tile % p.num_n_tiles;
+        const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
         const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, img = mt / (p.tiles_x * p.tiles_y);
         const int x0 = tx * p.bw, y0 = ty * p.bh, n0 = nt * BLOCK_N;
         for (int it = it0; it < it1; ++it) {
           const int tap = it / k_chunks, kc = it % k_chunks;
           int dy = 0, dx = 0;
           if (p.taps == 9) { dy = tap / 3 - 1; dx = tap % 3 - 1; }
-          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_wait_relaxed(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
           tma_load_4d(smem_a + stage * Cfg::kABytes, &tmap_a, &full_bar[stage], kc * BLOCK_K, x0 + dx, y0 + dy, img);
-          if constexpr (kCluster == 1) {
-            tma_load_3d(smem_b + stage * Cfg::kBBytes, &tmap_b, &full_bar[stage], kc * BLOCK_K, tap, n0);
-          } else {  // my slice of the weight tile goes to every CTA of the cluster
-            constexpr int kRows = BLOCK_N / kCluster;
-            tma_load_3d_mcast(smem_b + stage * Cfg::kBBytes + cta_rank * (kRows * BLOCK_K * 2), &tmap_b, &full_bar[stage],
-                              kc * BLOCK_K, tap, n0 + cta_rank * kRows, kMask);
-          }
+          tma_load_3d(smem_b + stage * Cfg::kBBytes, &tmap_b, &full_bar[stage], kc * BLOCK_K, tap, n0);
           if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===================== MMA issuer =====================
-      constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, BLOCK_N, 0, 0);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int item = first_item; item < num_tiles; item += item_stride) {
-        const int ks = item / num_out_tiles;
-        const int it0 = ks * k_iters / p.k_split, it1 = (ks + 1) * k_iters / p.k_split;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int it = it0; it < it1; ++it) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t a_desc = make_smem_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes), 1);
-          const uint64_t b_desc = make_smem_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes), 1);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / 16; ++k) {
-            // advance 16 bf16 = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
-            umma_ss(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (it > it0 || k > 0) ? 1u : 0u);
-          }
-          // frees the smem stage (in every CTA that multicasts into it) once the MMAs above have read it
-          if constexpr (kCluster == 1) umma_commit(&empty_bar[stage]);
-          else umma_commit_mcast(&empty_bar[stage], kMask);
-          if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full[acc]);  // accumulator ready for the epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  }
   } else {
-    // ===================== epilogue warps (TMEM -> regs -> global) =====================
-    // Two warps per TMEM lane quarter: warps (4+q) and (8+q) take the even / odd 32-column chunks of the tile.
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 216;");
-    const int quarter = warp & 3;            // TMEM lane quarter this warp may access
-    const int half = (warp - 4) >> 2;        // 0: even chunks, 1: odd chunks
-    const int r = quarter * 32 + lane;       // row inside the 128-row tile
-    constexpr int kChunks = BLOCK_N / 32;
-    int acc = 0; uint32_t acc_phase = 0;
-    for (int item = first_item; item < num_tiles; item += item_stride) {
-      const int tile = item % num_out_tiles;
-      const bool add_bias = item < num_out_tiles;  // K slice 0 carries the bias
-      const int mt = (tile / p.num_n_tiles) * kCluster + cta_rank, nt = tile % p.num_n_tiles;
+    // ===================== consumer warpgroups: wgmma main loop, then the epilogue =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cg = (warp - 4) >> 2;          // consumer warpgroup: tile rows [64 cg, 64 cg + 64)
+    const int wg_warp = warp & 3;            // warp inside the warpgroup
+    const int wg_tid = threadIdx.x & 127;
+    // epilogue mapping after the exchange: warp (wg_warp) takes rows 32 (wg_warp & 1) .. +32 of the warpgroup's 64 and
+    // the even (half 0) or odd (half 1) 32-column chunk of every 64-column pair
+    const int half = wg_warp >> 1;
+    const int r_loc = (wg_warp & 1) * 32 + lane;
+    const int r = cg * 64 + r_loc;           // row inside the 128-row tile
+    float* xch = xch_base + cg * 64 * XCH_STRIDE;
+    uint8_t* stage_buf = stage_base + (warp - 4) * 4096;
+    const int bar_id = 1 + cg;               // named barrier of this warpgroup (0 is __syncthreads)
+    constexpr int kAcc = BLOCK_N / 2;
+    int stage = 0; uint32_t phase = 0;
+    for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
+      const int tile = item % num_out_tiles, ks = item / num_out_tiles;
+      const int it0 = ks * k_iters / p.k_split, it1 = (ks + 1) * k_iters / p.k_split;
+      const bool add_bias = ks == 0;  // K slice 0 carries the bias
+      float acc[kAcc];
+#pragma unroll
+      for (int i = 0; i < kAcc; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int it = it0; it < it1; ++it) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t a_desc = make_smem_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes + cg * 64 * 128));
+        const uint64_t b_desc = make_smem_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes));
+        fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / 16; ++k) {
+          // advance 16 bf16 = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
+          if constexpr (BLOCK_N == 256) wgmma_ss_n256<0>(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+          else wgmma_ss_n128<0>(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the MMAs of the previous stage have read their operands: release that stage
+        fence_regs(acc);
+        if (prev >= 0 && wg_tid == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (prev >= 0 && wg_tid == 0) mbar_arrive(&empty_bar[prev]);
+
+      const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
       const int tx = mt % p.tiles_x, ty = (mt / p.tiles_x) % p.tiles_y, img = mt / (p.tiles_x * p.tiles_y);
       const int px = tx * p.bw + r % p.bw, py = ty * p.bh + r / p.bw;
       const bool row_ok = (px < p.W) && (py < p.H) && (mt < p.num_m_tiles);
       const int m = (img * p.H + py) * p.W + px;
-      const int n_valid = min(kChunks, (p.N - nt * BLOCK_N + 31) / 32);
-      ResChunk rc_cur, rc_next;
-      size_t off_cur = 0, off_next = 0;
-      uint8_t* stage = stage_base + (warp - 4) * 4096;
-      if (half < n_valid && !p.tma_epi) {  // residual operands of the first chunk are fetched while the MMAs still run
-        off_next = out_offset(p, m, nt * BLOCK_N + half * 32, img, py, px);
-        prefetch_res(p, rc_next, off_next, row_ok, lane);
-      }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
+      const int n_valid = min(BLOCK_N / 32, (p.N - nt * BLOCK_N + 31) / 32);
       float fin[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-      for (int c = half; c < n_valid; c += 2) {
-        const int col0 = nt * BLOCK_N + c * 32;
-        uint32_t raw[32];
-        tmem_ld32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BLOCK_N + c * 32, raw);
-        rc_cur = rc_next;
-        off_cur = off_next;
-        if (c + 2 < n_valid && !p.tma_epi) {
-          off_next = out_offset(p, m, col0 + 64, img, py, px);
-          prefetch_res(p, rc_next, off_next, row_ok, lane);
+#pragma unroll
+      for (int cp = 0; cp < BLOCK_N / 64; ++cp) {
+        // fragments of columns [64 cp, 64 cp + 64) -> exchange tile -> one row-chunk per thread
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");  // previous reads of the exchange tile are done
+        {
+          const int fr = wg_warp * 16 + (lane >> 2), fc = 2 * (lane & 3);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int jj = cp * 8 + j;
+            *reinterpret_cast<float2*>(xch + fr * XCH_STRIDE + 8 * j + fc) = make_float2(acc[4 * jj], acc[4 * jj + 1]);
+            *reinterpret_cast<float2*>(xch + (fr + 8) * XCH_STRIDE + 8 * j + fc) =
+                make_float2(acc[4 * jj + 2], acc[4 * jj + 3]);
+          }
         }
-        tmem_ld_wait();
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+        const int c = 2 * cp + half;
+        if (c >= n_valid) continue;
+        const int col0 = nt * BLOCK_N + c * 32;
         float v[32];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(raw[i]);
+        for (int i = 0; i < 8; ++i) {
+          const float4 t = *reinterpret_cast<const float4*>(xch + r_loc * XCH_STRIDE + half * 32 + 4 * i);
+          v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+        }
         if (epilogue_rows(p, v, m, col0, row_ok, fin, add_bias, w4_smem) && !(p.debug & 1)) {
           if (p.tma_epi) {
             const bool to_b = p.split_col > 0 && col0 >= p.split_col;
-            const int r0 = quarter * 32;  // first tile row of this warp
-            epilogue_tma(p, v, stage, lane, to_b ? &tmap_o0b : &tmap_o0, p.tma_epi == 2,
+            const int r0 = cg * 64 + (wg_warp & 1) * 32;  // first tile row of this warp
+            epilogue_tma(p, v, stage_buf, lane, to_b ? &tmap_o0b : &tmap_o0, p.tma_epi == 2,
                          to_b ? col0 - p.split_col : col0, tx * p.bw + (r0 & (p.bw - 1)), ty * p.bh + (r0 >> p.bw_log2),
                          mt < p.num_m_tiles ? img : p.NB);
           } else {
-            epilogue_store(p, v, rc_cur, stage, lane, m, col0, off_cur, row_ok);
+            const size_t off = out_offset(p, m, col0, img, py, px);
+            ResChunk rc;
+            prefetch_res(p, rc, off, row_ok, lane);
+            epilogue_store(p, v, rc, stage_buf, lane, m, col0, off, row_ok);
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
       if (p.epi == EPI_FINAL) {
         // combine the two half-row partial dot products, then postprocess
         // (fast3r/dust3r/heads/postprocess.py:16-64): pts = xyz/|xyz| * expm1(|xyz|), conf = 1+exp(c)
-        float* slot = fin_smem + (acc * 128 + r) * 4;
+        float* slot = fin_smem + r * 4;
         if (half == 1) { slot[0] = fin[0]; slot[1] = fin[1]; slot[2] = fin[2]; slot[3] = fin[3]; }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
         if (half == 0 && row_ok) {
           const float x = fin[0] + slot[0] + __ldg(p.b4 + 0), y = fin[1] + slot[1] + __ldg(p.b4 + 1);
           const float z = fin[2] + slot[2] + __ldg(p.b4 + 2), c = fin[3] + slot[3] + __ldg(p.b4 + 3);
@@ -467,61 +429,36 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           p.conf[m] = 1.f + expf(c);
         }
       }
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
     if (p.tma_epi && lane == 0) tma_store_wait_all();  // bulk stores of this warp are complete before the CTA retires
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (kCluster > 1) cluster_sync_all();  // no CTA leaves while its peer may still signal / multicast to it
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-  }
 }
 
-template <int BLOCK_N, int kCluster>
+template <int BLOCK_N>
 static cudaError_t launch_gemm_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
                                  const CUtensorMap& to0b, const GemmArgs& a, int num_sms, cudaStream_t stream) {
   using Cfg = GemmCfg<BLOCK_N>;
   {  // (per launch: the attribute is per device and one process may drive several GPUs)
-    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<BLOCK_N, kCluster>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::kSmemBytes);
     if (e != cudaSuccess) return e;
   }
-  const int items = ((a.num_m_tiles + kCluster - 1) / kCluster) * a.num_n_tiles * a.k_split;
-  const int max_clusters = num_sms / kCluster;
-  const int clusters = items < max_clusters ? items : max_clusters;
+  const int items = a.num_m_tiles * a.num_n_tiles * a.k_split;
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(clusters * kCluster);
+  cfg.gridDim = dim3(items < num_sms ? items : num_sms);
   cfg.blockDim = dim3(GEMM_THREADS);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;  // (always set, also for kCluster == 1)
-  attr[0].val.clusterDim.x = kCluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if (pdl_enabled()) {
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.numAttrs = 2;
-  }
-  return cudaLaunchKernelEx(&cfg, gemm_kernel<BLOCK_N, kCluster>, ta, tb, to0, to0b, a);
+  cfg.numAttrs = launch_attrs(attr, 1);
+  return cudaLaunchKernelEx(&cfg, gemm_kernel<BLOCK_N>, ta, tb, to0, to0b, a);
 }
 
-cudaError_t launch_gemm(int block_n, int cluster, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
+cudaError_t launch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
                         const CUtensorMap& to0b, const GemmArgs& a, int num_sms, cudaStream_t stream) {
-  if (block_n == 256) {
-    return cluster == 2 ? launch_gemm_t<256, 2>(ta, tb, to0, to0b, a, num_sms, stream)
-                        : launch_gemm_t<256, 1>(ta, tb, to0, to0b, a, num_sms, stream);
-  }
-  return cluster == 2 ? launch_gemm_t<128, 2>(ta, tb, to0, to0b, a, num_sms, stream)
-                      : launch_gemm_t<128, 1>(ta, tb, to0, to0b, a, num_sms, stream);
+  if (block_n == 256) return launch_gemm_t<256>(ta, tb, to0, to0b, a, num_sms, stream);
+  return launch_gemm_t<128>(ta, tb, to0, to0b, a, num_sms, stream);
 }
 
 }  // namespace f3r

@@ -1,12 +1,12 @@
-"""B200-native drop-in for ``fast3r.models.fast3r.Fast3R`` (reference: fast3r/models/fast3r.py:45-497).
+"""H100-native drop-in for ``fast3r.models.fast3r.Fast3R`` (reference: fast3r/models/fast3r.py:45-497).
 
 Same constructor dicts, same ``state_dict`` key schema (SURVEY.md §8(b)), same
 ``forward(views, profiling=False) -> list[dict]`` contract and the same host-side RNG consumption for the random
-image-index embedding — but every tensor op of the path runs in hand-written sm_100a kernels behind the C ABI
+image-index embedding — but every tensor op of the path runs in hand-written sm_90a kernels behind the C ABI
 (``libfast3r_b200.so``).  torch.nn modules below are parameter containers only (so checkpoints load unchanged);
 their ``forward`` is never called.  There is no PyTorch/CPU fallback: without the CUDA library this raises.
 
-Numerics: bf16 tensor-core operands, fp32 accumulation (TMEM), fp32 residual stream, fp32 LayerNorm/softmax
+Numerics: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream, fp32 LayerNorm/softmax
 statistics, fp32 outputs — closer to the reference's fp32 path than the reference's own bf16-autocast path
 (SURVEY.md Appendix B).
 """
@@ -264,10 +264,10 @@ def _sync(device) -> None:
 
 
 def _require_cuda(device) -> None:
-    """The product has exactly one compute path: the sm_100a kernels.  (tests/ replace this hook, together with
+    """The product has exactly one compute path: the sm_90a kernels.  (tests/ replace this hook, together with
     ``fast3r_b200.model.ops``, by a CPU emulator of the C ABI to exercise the host orchestration without a GPU.)"""
     if device.type != "cuda":
-        raise RuntimeError("fast3r_b200.Fast3R runs on CUDA (sm_100a) only; call model.to('cuda') first. "
+        raise RuntimeError("fast3r_b200.Fast3R runs on CUDA (sm_90a) only; call model.to('cuda') first. "
                            "There is no CPU fallback.")
     L.load()
 
@@ -493,7 +493,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
             x = torch.empty(M, D, dtype=F32, device=imgs.device)
             self._linear(x3, a0, P_["pe_w"], P_["pe_b"], out0=x)
             self._tap("patch_embed", x)
-            if not x3 and self._taps is None and ops.pick_kv_split(c * enc.num_heads * ((P + 255) // 256), (P + 127) // 128) == 1:
+            if not x3 and self._taps is None and ops.pick_kv_split(c * enc.num_heads * ((P + 127) // 128), (P + 127) // 128) == 1:
                 # all encoder blocks of this chunk in ONE library call (f3r_transformer_blocks: the same seven launches per
                 # block, issued by the C side with its own workspace carving)
                 ops.transformer_blocks(x, P_["enc"], batch=c, seq=P, heads=enc.num_heads, eps=1e-6, scale=64 ** -0.5, rope=rope)

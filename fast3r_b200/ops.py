@@ -136,13 +136,13 @@ def linear(a: torch.Tensor, wt: torch.Tensor, bias=None, **kw):
     return gemm(a, wt, w=a.numel() // a.shape[-1], bias=bias, **kw)
 
 
-NUM_SMS = 148
+NUM_SMS = 132
 
 
 def pick_kv_split(units: int, key_blocks: int, max_split: int = 8) -> int:
-    """Key slices per (batch, head, 256-row query tile) unit so that units * slices CTAs fill whole waves of the 148
-    SMs (one CTA per SM): minimises ceil(units*s / 148) / s; every slice keeps >= 16 key blocks (below that the extra
-    prologues and the merge pass cost more than the idle SMs, measured at N=4); 1 = no slicing."""
+    """Key slices per (batch, head, 128-row query tile) unit so that units * slices CTAs fill whole waves of the 132
+    SMs (one CTA per SM): minimises ceil(units*s / 132) / s; every slice keeps >= 16 key blocks (below that the extra
+    prologues and the merge pass cost more than the idle SMs); 1 = no slicing."""
     if units >= 3 * NUM_SMS:
         return 1
     best, best_cost = 1, None
@@ -194,7 +194,7 @@ def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: in
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(st)
     ns = kv_split if kv_split is not None else (
-        1 if lse is not None else pick_kv_split(batch * heads * ((sq + 255) // 256), (skv + 127) // 128))
+        1 if lse is not None else pick_kv_split(batch * heads * ((sq + 127) // 128), (skv + 127) // 128))
     if ns > 1:
         part_o = torch.empty(ns, batch * sq, heads * 64, dtype=F32, device=q.device)
         part_lse = torch.empty(ns, batch, heads, sq, dtype=F32, device=q.device)

@@ -58,7 +58,7 @@ class KVExchange:
     gather buffer (`kv_workspace()`); `attend()` starts the NCCL all-gather on a side stream and meanwhile attends the
     local queries to the LOCAL keys; when the gather has landed it attends to the key ranges of the other ranks and merges
     the partial results by their log-sum-exp (exact softmax over the union, f3r_attention_merge).  The exchange is hidden
-    behind the local-chunk attention and every launch is key-sliced to fill the 148 SMs (ops.pick_kv_split).
+    behind the local-chunk attention and every launch is key-sliced to fill the 132 SMs (ops.pick_kv_split).
     General path (batch > 1, uneven shards, parity precision, CPU emulator): all-gather, then one attention call."""
 
     def __init__(self, sp, batch: int, s_local: int, dim: int, rows: List[int]):
@@ -189,7 +189,7 @@ class KVExchange:
         sp.bytes_exchanged += self.buf.numel() * self.buf.element_size()
         S, sl = self.s_total, self.s_local
         lo, hi = sp.rank * sl, (sp.rank + 1) * sl
-        units = heads * ((sl + 255) // 256)
+        units = heads * ((sl + 127) // 128)
         # local keys first (straight from this rank's slot), then the other ranks' ranges of the gather buffer
         ranges = [(lo, sl)] + [r for r in ((0, lo), (hi, S - hi)) if r[1] > 0]
         splits = [ops.pick_kv_split(units, (n + 127) // 128) for _, n in ranges]

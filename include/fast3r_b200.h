@@ -1,4 +1,4 @@
-/* fast3r_b200 — C ABI of the B200-native Fast3R forward-pass kernels (libfast3r_b200.so).
+/* fast3r_b200 — C ABI of the H100-native (sm_90a) Fast3R forward-pass kernels (libfast3r_b200.so).
  *
  * Drop-in boundary for the single-forward-pass hot path of facebookresearch/fast3r
  * (CroCo encoder -> fusion decoder -> DPT heads).  The reference's only native precedent is the
@@ -31,7 +31,7 @@ enum { F3R_EPI_STORE = 0, F3R_EPI_ROPE = 1, F3R_EPI_IDXEMB = 2, F3R_EPI_CONVT = 
 enum { F3R_ACT_NONE = 0, F3R_ACT_RELU = 1, F3R_ACT_GELU = 2 };
 
 /* One fused GEMM / implicit-GEMM convolution:
- *   acc[m, n] = sum_{tap, k} A[pixel(m) + shift(tap), k] * Wt[n, tap, k]          (fp32 accumulation in TMEM)
+ *   acc[m, n] = sum_{tap, k} A[pixel(m) + shift(tap), k] * Wt[n, tap, k]          (fp32 accumulation in registers)
  *   v = acc + bias[n] (+ RoPE2D | + idx-embedding row) (+ res0[m,n]) (+ res1[m,n])
  *   out1[m,n] = bf16(relu(v))   (optional);   out0[m,n] = act(v) as bf16 or fp32 (optional)
  * Replaces: nn.Linear qkv/proj/fc1/fc2 (fast3r/croco/models/blocks.py:94-97,125-128), decoder_embed + image-index
@@ -90,7 +90,7 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream);
 int f3r_attention(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo, float* lse,
                   int32_t batch, int32_t heads, int32_t sq, int32_t skv, float scale, void* stream);
 
-/* Key-slice form of f3r_attention, for (a) filling the 148 SMs when batch*heads*ceil(sq/256) is small and (b) attending
+/* Key-slice form of f3r_attention, for (a) filling the SMs when batch*heads*ceil(sq/128) is small and (b) attending
  * to key ranges as they arrive over NVLink (sequence-parallel decoder, fast3r_b200/parallel.py): attends the queries to
  * the keys [kv_row0, kv_row0 + skv) of a kv buffer of kv_rows_total rows per batch, cut into n_split slices (one CTA each
  * per 256-row query tile); slice s writes its softmax-normalised fp32 output into part_o[part_base + s] (layout

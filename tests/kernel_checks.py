@@ -213,7 +213,7 @@ def check_attention_autosplit(batch=1, heads=4, sq=600, skv=4000, scale=0.16019,
     a = torch.zeros(batch * sq, D, dtype=torch.bfloat16, device="cuda")
     b = torch.zeros_like(a)
     ops.attention(q, kv, a, batch=batch, heads=heads, sq=sq, skv=skv, scale=scale, kv_split=1)
-    ns = ops.pick_kv_split(batch * heads * ((sq + 255) // 256), (skv + 127) // 128)
+    ns = ops.pick_kv_split(batch * heads * ((sq + 127) // 128), (skv + 127) // 128)
     ops.attention(q, kv, b, batch=batch, heads=heads, sq=sq, skv=skv, scale=scale)
     return rel(b, a), 3e-3, dict(auto_split=ns)
 

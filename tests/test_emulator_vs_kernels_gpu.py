@@ -1,5 +1,5 @@
 """The C-ABI emulator used by the CPU host-orchestration tests (tests/abi_emulator.py) must describe the real
-kernels: same call, same inputs, outputs compared (bf16 rounding tolerance).  Needs a B200."""
+kernels: same call, same inputs, outputs compared (bf16 rounding tolerance).  Needs an H100."""
 import pytest
 import torch
 

@@ -162,10 +162,10 @@ def test_sequence_parallel_host_logic_gloo(n_views, batch):
 
 
 def test_pick_kv_split_invariants():
-    """ops.pick_kv_split: key slicing only when it fills more of the 148 SMs, every slice keeps >= 16 key blocks, and the
-    measured shapes map to the measured choices (profiles/r02_notes.md)."""
+    """ops.pick_kv_split: key slicing only when it fills more of the 132 SMs, every slice keeps >= 16 key blocks, and the
+    decoder shapes of the sequence-parallel runs (16 heads, 128-row query tiles) map to fixed choices."""
     from fast3r_b200.ops import pick_kv_split, NUM_SMS
-    for units in (1, 16, 64, 148, 192, 368, 443, 444, 736, 1472, 23552):
+    for units in (1, 16, 64, 132, 192, 368, 395, 396, 736, 1472, 23552):
         for blocks in (1, 6, 15, 16, 23, 32, 92, 184, 1840):
             s = pick_kv_split(units, blocks)
             assert 1 <= s <= 8
@@ -174,9 +174,9 @@ def test_pick_kv_split_invariants():
                 assert s == 1
             waves = lambda k: -(-units * k // NUM_SMS) / k  # noqa: E731
             assert waves(s) <= waves(1) + 1e-9            # never worse than one slice
-    assert pick_kv_split(192, 184) == 3      # N=32 shard on 8 GPUs (2 waves at 65 % -> 4 waves of thirds)
-    assert pick_kv_split(368, 184) == 2      # 4 GPUs
-    assert pick_kv_split(1472, 184) == 1     # one GPU
+    assert pick_kv_split(192, 184) == 2      # 2 waves at 73 % -> 3 waves of halves at 97 %
+    assert pick_kv_split(368, 184) == 5      # 3 waves at 93 % -> 14 waves of fifths at 99.6 %
+    assert pick_kv_split(1472, 184) == 1     # 12 waves: never sliced (>= 3 waves)
     assert pick_kv_split(192, 23) == 1       # N=4: slices would be too short
 
 

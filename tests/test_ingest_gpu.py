@@ -1,5 +1,5 @@
 """Image ingest kernels (f3r_ingest_rgb8) against the CPU oracle (oracle/ingest_oracle.c, pinned against Pillow /
-torchvision / the reference's load_images by tests/test_ingest_cpu.py): bit-exact.  Needs a B200."""
+torchvision / the reference's load_images by tests/test_ingest_cpu.py): bit-exact.  Needs an H100."""
 import numpy as np
 import pytest
 import torch

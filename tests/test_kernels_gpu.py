@@ -1,4 +1,4 @@
-"""Each CUDA kernel (through the C ABI) vs a plain PyTorch fp32 reference of the same op.  Needs a B200."""
+"""Each CUDA kernel (through the C ABI) vs a plain PyTorch fp32 reference of the same op.  Needs an H100."""
 import pytest
 
 pytestmark = pytest.mark.gpu

@@ -1,5 +1,5 @@
 """End-to-end parity of the CUDA path against (a) the committed reference outputs (tests/golden, generated
-by the UNMODIFIED reference) and (b) the CPU oracle on the same seeded inputs.  Needs a B200.
+by the UNMODIFIED reference) and (b) the CPU oracle on the same seeded inputs.  Needs an H100.
 
 Tolerances (relative L2, stated per SURVEY.md §8(c) 'tolerance calibration'): the reference's OWN bf16-autocast
 path differs from its fp32 path by the amount stored in the fixture (``ref_bf16_vs_fp32_relL2``: 1.2e-2 on

@@ -1,4 +1,4 @@
-"""Sequence-parallel forward == single-GPU forward (needs >= 2 B200s; skipped otherwise)."""
+"""Sequence-parallel forward == single-GPU forward (needs >= 2 GPUs; skipped otherwise)."""
 import os
 import socket
 import subprocess

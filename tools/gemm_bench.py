@@ -1,4 +1,4 @@
-"""Times f3r_gemm on the decoder shapes (CUDA events, L2-flushed between reps).  Env knobs: F3R_GEMM_CLUSTER, F3R_GEMM_DEBUG."""
+"""Times f3r_gemm on the decoder shapes (CUDA events, L2-flushed between reps).  Env knob: F3R_GEMM_DEBUG."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -43,5 +43,5 @@ ops.attention(qq, kk, torch.empty(sq, D, dtype=bf, device=dev), batch=1, heads=1
 xf = r(2944, D, dt=f32, sc=1.0)
 ops.gemm_x3(xf, r(D, 1, 3 * D), w=2944, bias=r(D, dt=f32), out0=torch.empty(2944, D, dtype=f32, device=dev))   # split3 + x3 GEMM
 ops.attention_x3(r(2944, D, dt=f32, sc=1.0), r(2944, 2 * D, dt=f32, sc=1.0), torch.empty(2944, D, dtype=f32, device=dev),
-                 batch=1, heads=16, sq=2944, skv=2944, scale=0.16)           # attn_split + attention_x3
+                 batch=1, heads=16, sq=2944, skv=2944, scale=0.16)           # attn_split_kernel + attention_x3
 torch.cuda.synchronize()
