@@ -7,6 +7,14 @@
 // and used directly as the register A operand of O += P V (V consumed MN-major from shared memory, no transpose).
 // Softmax is exact online softmax in fp32 (exp2 domain) with lazy O rescaling: the running reference max is only
 // moved when the row max grows by more than 2^8.
+//
+// At head dim 64 the tensor pipe (256 MMA FLOP per score) and the MUFU ex2 (one per score) need the same time, so the
+// consumers overlap them (the intra-warpgroup pipelining of FlashAttention-3): S_{j+1} = Q K_{j+1}^T and O += P_j V_j
+// are issued back to back, the softmax of S_{j+1} runs while the PV is still on the tensor core, and only then is O
+// rescaled and P_{j+1} packed.  The two consumer warpgroups are not ordered against each other: a named-barrier
+// ping-pong (one warpgroup issues its GEMMs while the other is in its softmax) measured 2-4 % slower on top of this.
+// The arithmetic (ex2 inputs, order of the l and O updates, lazy-rescale decisions) is that of a loop that finishes one
+// key block before it starts the next, so the overlap does not change a bit of the result.
 #include "common.cuh"
 #include "f3r_kernels.h"
 
@@ -21,6 +29,78 @@ F3R_DEVICE float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
+}
+
+// S (64 rows x 128 keys of this warpgroup) = Q K^T, four k16 steps; committed as one wgmma group
+F3R_DEVICE void att_issue_s(float (&s)[64], uint64_t qd, const uint8_t* smem_k_stage) {
+  const uint64_t kd = make_smem_desc_sw128(smem_u32(smem_k_stage));
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wgmma_ss_n128<0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
+  wgmma_commit();
+}
+
+// O += P V, eight k16 steps of 16 keys (16 smem rows = 2048 B of V); committed as one wgmma group
+F3R_DEVICE void att_issue_pv(float (&o)[32], const uint32_t (&pa)[8][4], const uint8_t* smem_v_stage) {
+  const uint64_t vd = make_smem_desc_sw128(smem_u32(smem_v_stage));
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) wgmma_rs_n64<1>(o, pa[kk], vd + 128 * kk, 1u);
+  wgmma_commit();
+}
+
+// Online softmax of one key block, in place: s becomes exp2(S sl2 - m sl2).  Keys >= valid are masked.  Updates the
+// reference max and the row sums; the O rescale it decides (resc / alpha per row half) is applied by the caller once
+// no PV that accumulates into O is in flight.
+F3R_DEVICE void att_softmax(float (&s)[64], int valid, int cq, float sl2, float (&m_used)[2], float (&l)[2],
+                            bool (&resc)[2], float (&alpha)[2]) {
+  if (valid < 128) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i)
+      if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
+  }
+  float nm[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float mx = fmaxf(s[2 * hh], s[2 * hh + 1]);
+#pragma unroll
+    for (int jn = 1; jn < 16; ++jn) mx = fmaxf(mx, fmaxf(s[4 * jn + 2 * hh], s[4 * jn + 2 * hh + 1]));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    // lazy rescale: move the reference only if the max grew by more than 8 (log2 domain)
+    resc[hh] = (mx - m_used[hh]) * sl2 > 8.f;  // (-inf reference => true)
+    if (resc[hh]) {
+      alpha[hh] = ex2_approx((m_used[hh] - mx) * sl2);  // exp2(-inf) = 0 on the first block
+      m_used[hh] = mx;
+      l[hh] *= alpha[hh];
+    }
+    nm[hh] = -m_used[hh] * sl2;
+  }
+  // k-step kk of the PV covers key columns [16 kk, 16 kk + 16): s[8 kk + 2 r + {0, 1}], row half r & 1
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int i = 8 * kk + 2 * r, hh = r & 1;
+      const float e0 = ex2_approx(fmaf(s[i], sl2, nm[hh])), e1 = ex2_approx(fmaf(s[i + 1], sl2, nm[hh]));
+      l[hh] += e0 + e1;
+      s[i] = e0;
+      s[i + 1] = e1;
+    }
+  }
+}
+
+// After the last PV that read pa has landed: O *= alpha where the softmax moved the reference, then P -> bf16 A fragments
+F3R_DEVICE void att_rescale_pack(float (&o)[32], uint32_t (&pa)[8][4], const float (&s)[64], const bool (&resc)[2],
+                                 const float (&alpha)[2]) {
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh)
+    if (resc[hh]) {
+#pragma unroll
+      for (int jn = 0; jn < 8; ++jn) { o[4 * jn + 2 * hh] *= alpha[hh]; o[4 * jn + 2 * hh + 1] *= alpha[hh]; }
+    }
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) pa[kk][r] = pack_bf16(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
 }
 
 __global__ void __launch_bounds__(ATT_THREADS, 1)
@@ -100,76 +180,58 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     float o[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    float s[64];         // S of the block in softmax, then its exponentials until they are packed
+    uint32_t pa[8][4];   // P of the block whose PV is in flight (bf16 A fragments)
+    bool resc[2];        // O rescale decided by the latest softmax ...
+    float alpha[2];      // ... and its factor
     const uint64_t qd = make_smem_desc_sw128(smem_u32(smem_q + cg * 64 * 128));
+    // keys valid in key block j of this CTA: only the last block of the launch's key range is partial
+    auto valid_keys = [&](int j) { return j0 + j == nkv_all - 1 ? p.skv - (j0 + j) * 128 : 128; };
     mbar_wait(q_full, 0);
 
-    for (int j = 0; j < nkv; ++j) {
-      const int st = j % ATT_STAGES;
-      const uint32_t ph = (j / ATT_STAGES) & 1;
-      float s[64];
-      mbar_wait(&k_full[st], ph);
-      {
-        const uint64_t kd = make_smem_desc_sw128(smem_u32(smem_k + st * ATT_TILE_BYTES));
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_ss_n128<0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(s);
-      }
-      if (wg_tid == 0) mbar_arrive(&k_empty[st]);
+    // block 0: S_0 and its softmax
+    mbar_wait(&k_full[0], 0);
+    wgmma_fence();
+    att_issue_s(s, qd, smem_k);
+    wgmma_wait<0>();
+    fence_regs(s);
+    if (wg_tid == 0) mbar_arrive(&k_empty[0]);
+    att_softmax(s, valid_keys(0), cq, sl2, m_used, l, resc, alpha);
 
-      if (j0 + j == nkv_all - 1) {  // last key block of the launch's range: keys past its end are masked
-        const int valid = p.skv - (j0 + j) * 128;
-        if (valid < 128) {
-#pragma unroll
-          for (int i = 0; i < 64; ++i)
-            if (8 * (i >> 2) + cq + (i & 1) >= valid) s[i] = -INFINITY;
-        }
-      }
-      float nm[2];
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        float mx = fmaxf(s[2 * hh], s[2 * hh + 1]);
-#pragma unroll
-        for (int jn = 1; jn < 16; ++jn) mx = fmaxf(mx, fmaxf(s[4 * jn + 2 * hh], s[4 * jn + 2 * hh + 1]));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        // lazy rescale: move the reference only if the max grew by more than 8 (log2 domain)
-        if ((mx - m_used[hh]) * sl2 > 8.f) {  // (-inf reference => true)
-          const float alpha = ex2_approx((m_used[hh] - mx) * sl2);  // exp2(-inf) = 0 on the first block
-          m_used[hh] = mx;
-          l[hh] *= alpha;
-#pragma unroll
-          for (int jn = 0; jn < 8; ++jn) { o[4 * jn + 2 * hh] *= alpha; o[4 * jn + 2 * hh + 1] *= alpha; }
-        }
-        nm[hh] = -m_used[hh] * sl2;
-      }
-      // P = exp2(S sl2 - m sl2), packed to bf16 A fragments: k-step kk covers key columns [16 kk, 16 kk + 16)
-      uint32_t pa[8][4];
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int i = 8 * kk + 2 * r, hh = r & 1;
-          const float e0 = ex2_approx(fmaf(s[i], sl2, nm[hh])), e1 = ex2_approx(fmaf(s[i + 1], sl2, nm[hh]));
-          l[hh] += e0 + e1;
-          pa[kk][r] = pack_bf16(e0, e1);
-        }
-      }
-      mbar_wait(&v_full[st], ph);
-      {
-        const uint64_t vd = make_smem_desc_sw128(smem_u32(smem_v + st * ATT_TILE_BYTES));
-        fence_regs(o);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)  // 16 keys per MMA: 16 smem rows (2048 B) of V
-          wgmma_rs_n64<1>(o, pa[kk], vd + 128 * kk, 1u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(o);
-      }
-      if (wg_tid == 0) mbar_arrive(&v_empty[st]);
+    // steady state: on entry the softmax of S_j is done and PV_{j-1} may be in flight.  S_{j+1} and PV_j go out
+    // together and the softmax of S_{j+1} runs under PV_j.  The wait for PV_j sits at the top of the next trip, behind
+    // the mbarrier polls: the instruction scheduler hoists a wgmma wait above independent math in the same basic block,
+    // which would put the softmax back behind the PV.
+    for (int j = 0; j + 1 < nkv; ++j) {
+      const int sk = (j + 1) % ATT_STAGES, sv = j % ATT_STAGES;
+      mbar_wait(&k_full[sk], ((j + 1) / ATT_STAGES) & 1);
+      mbar_wait(&v_full[sv], (j / ATT_STAGES) & 1);
+      wgmma_wait<0>();  // PV_{j-1} has landed: O may be rescaled and the P registers rewritten
+      fence_regs(o);
+      if (j > 0 && wg_tid == 0) mbar_arrive(&v_empty[(j - 1) % ATT_STAGES]);
+      att_rescale_pack(o, pa, s, resc, alpha);
+      wgmma_fence();
+      att_issue_s(s, qd, smem_k + sk * ATT_TILE_BYTES);
+      att_issue_pv(o, pa, smem_v + sv * ATT_TILE_BYTES);
+      wgmma_wait<1>();  // S_{j+1} has landed (groups complete in order)
+      fence_regs(s);
+      if (wg_tid == 0) mbar_arrive(&k_empty[sk]);
+      att_softmax(s, valid_keys(j + 1), cq, sl2, m_used, l, resc, alpha);
+    }
+
+    // last block: PV only
+    {
+      const int sv = (nkv - 1) % ATT_STAGES;
+      mbar_wait(&v_full[sv], ((nkv - 1) / ATT_STAGES) & 1);
+      wgmma_wait<0>();
+      fence_regs(o);
+      if (nkv > 1 && wg_tid == 0) mbar_arrive(&v_empty[(nkv - 2) % ATT_STAGES]);
+      att_rescale_pack(o, pa, s, resc, alpha);
+      wgmma_fence();
+      att_issue_pv(o, pa, smem_v + sv * ATT_TILE_BYTES);
+      wgmma_wait<0>();
+      fence_regs(o);
+      if (wg_tid == 0) mbar_arrive(&v_empty[sv]);
     }
 
     // ---- epilogue: O / l -> global
