@@ -1,18 +1,22 @@
 // FlashAttention-style forward for head_dim 64 on sm_90a: softmax(scale * Q K^T) V, non-causal, no mask
 // (fast3r/croco/models/blocks.py:135-194; encoder: batch = views, S = P; fusion decoder: batch = B, S = N*P).
 //
-// One CTA owns 128 query rows of one (batch, head) and streams all keys of its range in blocks of 128.  Warpgroup 0
-// is the TMA producer (Q once, K/V blocks into a 128B-swizzled smem ring); warpgroups 1 and 2 each own 64 query rows:
-// S = Q K^T is a wgmma with both operands in shared memory (S stays in registers), P is packed to bf16 in registers
-// and used directly as the register A operand of O += P V (V consumed MN-major from shared memory, no transpose).
+// One CTA owns ATT_Q_TILE = 192 query rows of one (batch, head) and streams all keys of its range in blocks of 128.
+// Warpgroup 0 is the TMA producer (Q once, K/V blocks into a 128B-swizzled smem ring); warpgroups 1, 2 and 3 each own
+// 64 query rows, so every K/V byte brought in from L2 serves 192 rows: S = Q K^T is a wgmma with both operands in shared
+// memory (S stays in registers), P is packed to bf16 in registers and used directly as the register A operand of
+// O += P V (V consumed MN-major from shared memory, no transpose).  Every consumer warpgroup runs the whole key loop
+// and releases every stage, also when all its rows lie past sq (the producer waits for three releases per stage); only
+// its stores are masked.
 // Softmax is exact online softmax in fp32 (exp2 domain) with lazy O rescaling: the running reference max is only
 // moved when the row max grows by more than 2^8.
 //
 // At head dim 64 the tensor pipe (256 MMA FLOP per score) and the MUFU ex2 (one per score) need the same time, so the
 // consumers overlap them (the intra-warpgroup pipelining of FlashAttention-3): S_{j+1} = Q K_{j+1}^T and O += P_j V_j
 // are issued back to back, the softmax of S_{j+1} runs while the PV is still on the tensor core, and only then is O
-// rescaled and P_{j+1} packed.  The two consumer warpgroups are not ordered against each other: a named-barrier
-// ping-pong (one warpgroup issues its GEMMs while the other is in its softmax) measured 2-4 % slower on top of this.
+// rescaled and P_{j+1} packed.  The consumer warpgroups are not ordered against each other: a named-barrier
+// ping-pong (one warpgroup issues its GEMMs while the other is in its softmax) measured 2-4 % slower on top of this
+// with two consumer warpgroups.
 // The arithmetic (ex2 inputs, order of the l and O updates, lazy-rescale decisions) is that of a loop that finishes one
 // key block before it starts the next, so the overlap does not change a bit of the result.
 #include "common.cuh"
@@ -20,10 +24,14 @@
 
 namespace f3r {
 
-constexpr int ATT_THREADS = 384;
+constexpr int ATT_CONSUMERS = ATT_Q_TILE / 64;          // consumer warpgroups, 64 query rows each
+constexpr int ATT_THREADS = 128 * (1 + ATT_CONSUMERS);   // + the producer warpgroup
 constexpr int ATT_STAGES = 3;
-constexpr int ATT_TILE_BYTES = 128 * 64 * 2;  // 16 KB: 128 rows x 64 bf16
-constexpr int ATT_SMEM_BYTES = (1 + 2 * ATT_STAGES) * ATT_TILE_BYTES + 1024 + 256;
+constexpr int ATT_TILE_BYTES = 128 * 64 * 2;             // 16 KB: one K or V block, 128 keys x 64 bf16
+constexpr int ATT_Q_BYTES = ATT_Q_TILE * 64 * 2;         // 24 KB
+constexpr int ATT_SMEM_BYTES = ATT_Q_BYTES + 2 * ATT_STAGES * ATT_TILE_BYTES + 1024 + 256;
+static_assert(ATT_Q_TILE == 192, "the register split below (setmaxnreg 24 / 160) is sized for three consumer warpgroups");
+static_assert(ATT_Q_BYTES % 1024 == 0, "the K/V ring after Q must stay 1024-byte aligned (128B swizzle atoms)");
 
 F3R_DEVICE float ex2_approx(float x) {
   float y;
@@ -108,8 +116,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                  const __grid_constant__ AttnArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_q = smem;                                   // 1 tile
-  uint8_t* smem_k = smem + ATT_TILE_BYTES;                  // ATT_STAGES tiles
+  uint8_t* smem_q = smem;                                   // ATT_Q_TILE rows
+  uint8_t* smem_k = smem + ATT_Q_BYTES;                     // ATT_STAGES tiles
   uint8_t* smem_v = smem_k + ATT_STAGES * ATT_TILE_BYTES;   // ATT_STAGES tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_v + ATT_STAGES * ATT_TILE_BYTES);
   uint64_t* q_full = bars;                       // 1
@@ -121,7 +129,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // work item = (unit = (batch, head, 128-row query tile), split = slice of the key blocks of this launch's key range)
+  // work item = (unit = (batch, head, query tile of ATT_Q_TILE rows), split = slice of the key blocks of this launch's
+  // key range)
   const int unit = blockIdx.x / p.n_split;
   const int split = blockIdx.x % p.n_split;
   const int qt = unit % p.q_tiles;
@@ -138,8 +147,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     tma_prefetch_desc(&tmap_kv);
     mbar_init(q_full, 1);
     for (int s = 0; s < ATT_STAGES; ++s) {
-      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 2);  // released by both consumer warpgroups
-      mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 2);
+      mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], ATT_CONSUMERS);  // released by every consumer warpgroup
+      mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], ATT_CONSUMERS);
     }
     fence_barrier_init();
   }
@@ -148,11 +157,12 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   pdl_launch_dependents();
 
   if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");   // 128 x 40 + 256 x 232 <= 64K registers
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");   // 128 x 24 + 384 x 160 <= 64K registers
     if (warp == 0 && lane == 0) {
       // ===================== TMA producer =====================
-      mbar_arrive_expect_tx(q_full, ATT_TILE_BYTES);
-      tma_load_3d(smem_q, &tmap_q, q_full, h * 64, qt * 128, b);
+      // (Q rows past sq are zero-filled by the TMA unit and still count towards the transaction bytes)
+      mbar_arrive_expect_tx(q_full, ATT_Q_BYTES);
+      tma_load_3d(smem_q, &tmap_q, q_full, h * 64, qt * ATT_Q_TILE, b);
       int stage = 0; uint32_t phase = 0;
       for (int j = 0; j < nkv; ++j) {
         mbar_wait_relaxed(&k_empty[stage], phase ^ 1);
@@ -169,10 +179,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     // ===================== consumer warpgroups: 64 query rows each =====================
     // accumulator fragments (common.cuh): this thread holds rows rw + 8 hh (hh = 0, 1) and, in every 8-column group jn,
     // the columns 8 jn + 2 (lane % 4) + {0, 1}
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 160;");
     const int cg = (warp - 4) >> 2;
     const int wg_tid = threadIdx.x & 127;
-    const int rw = cg * 64 + (warp & 3) * 16 + (lane >> 2);  // first of the thread's two rows in the 128-row tile
+    const int rw = cg * 64 + (warp & 3) * 16 + (lane >> 2);  // first of the thread's two rows in the query tile
     const int cq = 2 * (lane & 3);
     const float sl2 = p.scale_log2;
     float m_used[2] = {-INFINITY, -INFINITY};  // raw-score reference max the exponentials are taken against
@@ -242,7 +252,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     }
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
-      const int q = qt * 128 + rw + 8 * hh;
+      const int q = qt * ATT_Q_TILE + rw + 8 * hh;
       if (q >= p.sq) continue;
       const float inv = 1.f / l[hh];
       const float lse = m_used[hh] * sl2 * 0.69314718056f + logf(l[hh]);

@@ -224,7 +224,7 @@ static int attention_impl(const char* what, const void* q, int32_t ldq, const vo
     const uint64_t dims[3] = {static_cast<uint64_t>(heads) * 64, static_cast<uint64_t>(sq),
                               static_cast<uint64_t>(batch)};
     const uint64_t str[2] = {static_cast<uint64_t>(ldq) * 2, static_cast<uint64_t>(ldq) * 2 * sq};
-    const uint32_t box[3] = {64, 128, 1};
+    const uint32_t box[3] = {64, f3r::ATT_Q_TILE, 1};
     if (make_tmap(&tq, q, 3, dims, str, box)) return 1;
   }
   {
@@ -237,7 +237,7 @@ static int attention_impl(const char* what, const void* q, int32_t ldq, const vo
   f3r::AttnArgs a;
   memset(&a, 0, sizeof(a));
   a.batch = batch; a.heads = heads; a.sq = sq; a.skv = skv;
-  a.q_tiles = (sq + 127) / 128;
+  a.q_tiles = (sq + f3r::ATT_Q_TILE - 1) / f3r::ATT_Q_TILE;
   a.scale_log2 = scale * 1.4426950408889634f;
   a.ldo = ldo; a.out = out; a.lse = lse;
   a.kv_row0 = kv_row0; a.n_split = n_split; a.part_base = part_base; a.part_o = part_o; a.part_lse = part_lse;

@@ -48,9 +48,12 @@ struct GemmArgs {
 cudaError_t launch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
                         const CUtensorMap& to0b, const GemmArgs& a, int num_sms, cudaStream_t stream);
 
+// query rows per CTA of attention_kernel: three consumer warpgroups of 64 rows (ops.ATT_Q_TILE on the Python side)
+constexpr int ATT_Q_TILE = 192;
+
 struct AttnArgs {
   int batch, heads, sq, skv;  // per-batch query / key lengths
-  int q_tiles;                // ceil(sq / 128)
+  int q_tiles;                // ceil(sq / ATT_Q_TILE) (attention_x3: ceil(sq / 128))
   float scale_log2;           // softmax scale * log2(e)
   int ldo;                    // row stride of out (elements)
   void* out;                  // bf16 [batch*sq, ldo], head h at columns h*64

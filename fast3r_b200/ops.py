@@ -137,11 +137,17 @@ def linear(a: torch.Tensor, wt: torch.Tensor, bias=None, **kw):
 
 
 NUM_SMS = 132
+ATT_Q_TILE = 192  # query rows per attention CTA (ATT_Q_TILE in csrc/f3r_kernels.h)
+
+
+def attention_units(batch: int, heads: int, sq: int) -> int:
+    """(batch, head, query tile) work units of one attention launch: its CTA count before key slicing."""
+    return batch * heads * -(-sq // ATT_Q_TILE)
 
 
 def pick_kv_split(units: int, key_blocks: int, max_split: int = 8) -> int:
-    """Key slices per (batch, head, 128-row query tile) unit so that units * slices CTAs fill whole waves of the 132
-    SMs (one CTA per SM): minimises ceil(units*s / 132) / s; every slice keeps >= 16 key blocks (below that the extra
+    """Key slices per (batch, head, query tile) unit (attention_units) so that units * slices CTAs fill whole waves of
+    the 132 SMs (one CTA per SM): minimises ceil(units*s / 132) / s; every slice keeps >= 16 key blocks (below that the extra
     prologues and the merge pass cost more than the idle SMs); 1 = no slicing."""
     if units >= 3 * NUM_SMS:
         return 1
@@ -194,7 +200,7 @@ def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: in
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(st)
     ns = kv_split if kv_split is not None else (
-        1 if lse is not None else pick_kv_split(batch * heads * ((sq + 127) // 128), (skv + 127) // 128))
+        1 if lse is not None else pick_kv_split(attention_units(batch, heads, sq), (skv + 127) // 128))
     if ns > 1:
         part_o = torch.empty(ns, batch * sq, heads * 64, dtype=F32, device=q.device)
         part_lse = torch.empty(ns, batch, heads, sq, dtype=F32, device=q.device)

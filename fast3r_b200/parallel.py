@@ -15,6 +15,8 @@ from typing import List, Tuple
 import torch
 import torch.distributed as dist
 
+from .ops import attention_units
+
 
 def _all_gather_into(out: torch.Tensor, inp: torch.Tensor, group=None) -> None:
     """dist.all_gather_into_tensor that also works for CUDA tensors over a gloo group (staged through the host): lets two
@@ -189,7 +191,7 @@ class KVExchange:
         sp.bytes_exchanged += self.buf.numel() * self.buf.element_size()
         S, sl = self.s_total, self.s_local
         lo, hi = sp.rank * sl, (sp.rank + 1) * sl
-        units = heads * ((sl + 127) // 128)
+        units = attention_units(1, heads, sl)
         # local keys first (straight from this rank's slot), then the other ranks' ranges of the gather buffer
         ranges = [(lo, sl)] + [r for r in ((0, lo), (hi, S - hi)) if r[1] > 0]
         splits = [ops.pick_kv_split(units, (n + 127) // 128) for _, n in ranges]
