@@ -15,6 +15,7 @@ from __future__ import annotations
 import math
 import time
 from copy import deepcopy
+from itertools import accumulate
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -188,74 +189,105 @@ class PixelwiseTaskWithDPT(nn.Module):
 
 
 # --------------------------------------------------------------------------- packed (device) weights
-# Every GEMM weight is packed as [N_out, taps, K] with K contiguous (include/fast3r_b200.h).  Fast path: bf16.
-# Parity path ("fp32"): [Whi | Whi | Wlo] along K (3K wide), matching the [hi | lo | hi] split of the activation, so
-# the same kernel accumulates hi*hi + lo*hi + hi*lo in fp32 (fp32-level products on the bf16 tensor pipe).
-def _pk(w: torch.Tensor, x3: bool) -> torch.Tensor:
-    w = w.detach().to(F32)
-    hi = w.to(BF16)
-    if not x3:
-        return hi.contiguous()
-    lo = (w - hi.float()).to(BF16)
-    return torch.cat([hi, hi, lo], dim=-1).contiguous()
+# Every GEMM weight is packed as [N_out, taps, K] with K contiguous (include/fast3r_b200.h).
+class _Packed:
+    """Weights packed for one numeric path, which they carry along with the GEMM dispatch of that path.
+    ``precision`` "bf16" (fast path): bf16 weights and activations.  "fp32" (parity path): fp32 activations, which the
+    GEMM splits on the fly into bf16 [hi | lo | hi] along K, against weights packed as [Whi | Whi | Wlo] (3K wide), so
+    the same kernel accumulates hi*hi + lo*hi + hi*lo in fp32 (fp32-level products on the bf16 tensor pipe)."""
 
+    def __init__(self, precision: str):
+        self.x3 = precision == "fp32"
+        self.adt = F32 if self.x3 else BF16  # dtype of the activations that feed a GEMM
 
-def _w_lin(m, x3=False) -> torch.Tensor:
-    return _pk(m.weight.detach().reshape(m.weight.shape[0], 1, -1), x3)
+    def _pk(self, w: torch.Tensor) -> torch.Tensor:
+        w = w.detach().to(F32)
+        hi = w.to(BF16)
+        if not self.x3:
+            return hi.contiguous()
+        lo = (w - hi.float()).to(BF16)
+        return torch.cat([hi, hi, lo], dim=-1).contiguous()
 
+    def _lin(self, m) -> torch.Tensor:  # linear (out,in), 1x1 or patch conv (out,in,kh,kw) -> (out, 1, in*kh*kw)
+        return self._pk(m.weight.detach().reshape(m.weight.shape[0], 1, -1))
 
-def _w_conv3(m, x3=False) -> torch.Tensor:  # (out,in,3,3) -> (out, 9, in)
-    w = m.weight.detach()
-    return _pk(w.permute(0, 2, 3, 1).reshape(w.shape[0], 9, w.shape[1]), x3)
+    def _conv3(self, m) -> torch.Tensor:  # (out,in,3,3) -> (out, 9, in)
+        w = m.weight.detach()
+        return self._pk(w.permute(0, 2, 3, 1).reshape(w.shape[0], 9, w.shape[1]))
 
+    def _convt(self, m) -> torch.Tensor:  # (in,out,k,k) -> ((i*k+j)*out + o, 1, in)
+        w = m.weight.detach()
+        k = w.shape[2]
+        return self._pk(w.permute(2, 3, 1, 0).reshape(k * k * w.shape[1], 1, w.shape[0]))
 
-def _w_convt(m, x3=False) -> torch.Tensor:  # (in,out,k,k) -> ((i*k+j)*out + o, 1, in)
-    w = m.weight.detach()
-    k = w.shape[2]
-    return _pk(w.permute(2, 3, 1, 0).reshape(k * k * w.shape[1], 1, w.shape[0]), x3)
+    def gemm(self, a, wt, *, a_relu=False, a_relu_src=None, **kw):
+        """``a``: an ``adt`` activation.  ``a_relu`` multiplies relu(a) instead: the parity path folds the ReLU into the
+        operand split, the fast path reads the bf16 copy ``a_relu_src`` that the producing GEMM stored."""
+        if self.x3:
+            return ops.gemm_x3(a, wt, a_relu=a_relu, **kw)
+        return ops.gemm(a_relu_src if a_relu else a, wt, **kw)
 
-
-def _w_lin2d(m, x3=False) -> torch.Tensor:  # 1x1 conv (out,in,1,1) -> (out,1,in)
-    w = m.weight.detach()
-    return _pk(w.reshape(w.shape[0], 1, w.shape[1]), x3)
+    def linear(self, a, wt, bias=None, **kw):
+        return self.gemm(a, wt, w=a.numel() // a.shape[-1], bias=bias, **kw)
 
 
 def _f32(t) -> Optional[torch.Tensor]:
     return None if t is None else t.detach().to(F32).contiguous()
 
 
-class _BlockW:
-    def __init__(self, blk: _Block, x3=False):
+class _BlockW(_Packed):
+    def __init__(self, blk: _Block, precision="bf16"):
+        super().__init__(precision)
         self.n1w, self.n1b = _f32(blk.norm1.weight), _f32(blk.norm1.bias)
         self.n2w, self.n2b = _f32(blk.norm2.weight), _f32(blk.norm2.bias)
-        self.qkv_w, self.qkv_b = _w_lin(blk.attn.qkv, x3), _f32(blk.attn.qkv.bias)
-        self.proj_w, self.proj_b = _w_lin(blk.attn.proj, x3), _f32(blk.attn.proj.bias)
-        self.fc1_w, self.fc1_b = _w_lin(blk.mlp.fc1, x3), _f32(blk.mlp.fc1.bias)
-        self.fc2_w, self.fc2_b = _w_lin(blk.mlp.fc2, x3), _f32(blk.mlp.fc2.bias)
+        self.qkv_w, self.qkv_b = self._lin(blk.attn.qkv), _f32(blk.attn.qkv.bias)
+        self.proj_w, self.proj_b = self._lin(blk.attn.proj), _f32(blk.attn.proj.bias)
+        self.fc1_w, self.fc1_b = self._lin(blk.mlp.fc1), _f32(blk.mlp.fc1.bias)
+        self.fc2_w, self.fc2_b = self._lin(blk.mlp.fc2), _f32(blk.mlp.fc2.bias)
 
 
-class _DPTW:
-    def __init__(self, dpt: _DPT, x3=False):
+class _DPTW(_Packed):
+    def __init__(self, dpt: _DPT, precision="bf16"):
+        super().__init__(precision)
         ap = dpt.act_postprocess
-        self.ap0 = (_w_lin2d(ap[0][0], x3), _f32(ap[0][0].bias), _w_convt(ap[0][1], x3), _f32(ap[0][1].bias))
-        self.ap1 = (_w_lin2d(ap[1][0], x3), _f32(ap[1][0].bias), _w_convt(ap[1][1], x3), _f32(ap[1][1].bias))
-        self.ap2 = (_w_lin2d(ap[2][0], x3), _f32(ap[2][0].bias))
-        w31 = _w_conv3(ap[3][1], x3)  # stride-2 conv runs as im2col + linear: (out, 9, C') -> (out, 1, 9*C')
-        self.ap3 = (_w_lin2d(ap[3][0], x3), _f32(ap[3][0].bias), w31.reshape(w31.shape[0], 1, -1), _f32(ap[3][1].bias))
-        self.rn = [_w_conv3(m, x3) for m in dpt.scratch.layer_rn]
+        self.ap0 = (self._lin(ap[0][0]), _f32(ap[0][0].bias), self._convt(ap[0][1]), _f32(ap[0][1].bias))
+        self.ap1 = (self._lin(ap[1][0]), _f32(ap[1][0].bias), self._convt(ap[1][1]), _f32(ap[1][1].bias))
+        self.ap2 = (self._lin(ap[2][0]), _f32(ap[2][0].bias))
+        w31 = self._conv3(ap[3][1])  # stride-2 conv runs as im2col + linear: (out, 9, C') -> (out, 1, 9*C')
+        self.ap3 = (self._lin(ap[3][0]), _f32(ap[3][0].bias), w31.reshape(w31.shape[0], 1, -1), _f32(ap[3][1].bias))
+        self.rn = [self._conv3(m) for m in dpt.scratch.layer_rn]
         self.fus = {}
         for i in range(1, 5):
             f = getattr(dpt.scratch, f"refinenet{i}")
             self.fus[i] = dict(
-                out_w=_w_lin2d(f.out_conv, x3), out_b=_f32(f.out_conv.bias),
-                r1=(_w_conv3(f.resConfUnit1.conv1, x3), _f32(f.resConfUnit1.conv1.bias),
-                    _w_conv3(f.resConfUnit1.conv2, x3), _f32(f.resConfUnit1.conv2.bias)),
-                r2=(_w_conv3(f.resConfUnit2.conv1, x3), _f32(f.resConfUnit2.conv1.bias),
-                    _w_conv3(f.resConfUnit2.conv2, x3), _f32(f.resConfUnit2.conv2.bias)))
-        self.h0 = (_w_conv3(dpt.head[0], x3), _f32(dpt.head[0].bias))
-        self.h2 = (_w_conv3(dpt.head[2], x3), _f32(dpt.head[2].bias))
+                out_w=self._lin(f.out_conv), out_b=_f32(f.out_conv.bias),
+                r1=(self._conv3(f.resConfUnit1.conv1), _f32(f.resConfUnit1.conv1.bias),
+                    self._conv3(f.resConfUnit1.conv2), _f32(f.resConfUnit1.conv2.bias)),
+                r2=(self._conv3(f.resConfUnit2.conv1), _f32(f.resConfUnit2.conv1.bias),
+                    self._conv3(f.resConfUnit2.conv2), _f32(f.resConfUnit2.conv2.bias)))
+        self.h0 = (self._conv3(dpt.head[0]), _f32(dpt.head[0].bias))
+        self.h2 = (self._conv3(dpt.head[2]), _f32(dpt.head[2].bias))
         self.w4 = dpt.head[4].weight.detach().to(F32).reshape(dpt.head[4].weight.shape[0], -1).contiguous()
         self.b4 = _f32(dpt.head[4].bias)
+
+
+class _ModelW(_Packed):
+    def __init__(self, model: "Fast3R", precision: str, device):
+        super().__init__(precision)
+        enc, dec = model.encoder, model.decoder
+        self.pe_w, self.pe_b = self._lin(enc.patch_embed.proj), _f32(enc.patch_embed.proj.bias)
+        self.enc = [_BlockW(b, precision) for b in enc.enc_blocks]
+        self.enc_nw, self.enc_nb = _f32(enc.enc_norm.weight), _f32(enc.enc_norm.bias)
+        self.de_w, self.de_b = self._lin(dec.decoder_embed), _f32(dec.decoder_embed.bias)
+        self.dec = [_BlockW(b, precision) for b in dec.dec_blocks]
+        self.dec_nw, self.dec_nb = _f32(dec.dec_norm.weight), _f32(dec.dec_norm.bias)
+        self.table = dec.image_idx_emb.detach().to(device=device, dtype=F32).contiguous()
+        self.head = _DPTW(model.downstream_head.dpt, precision)
+        local = model.downstream_head_local
+        self.head_local = _DPTW(local.dpt, precision) if local is not None else None
+        j = torch.arange(16, dtype=torch.float32)
+        ang = torch.arange(256, dtype=torch.float32)[:, None] * (1.0 / (enc.rope_base ** (j / 16.0)))[None]
+        self.rope_cos, self.rope_sin = ang.cos().contiguous().to(device), ang.sin().contiguous().to(device)
 
 
 def _sync(device) -> None:
@@ -403,8 +435,8 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
     def _signature(self):
         return tuple((p.data_ptr(), p._version) for p in self.parameters())
 
-    def _pack(self, device, x3=False):
-        mode = "fp32" if x3 else "bf16"
+    def _pack(self, device) -> _ModelW:
+        mode = self.precision
         sig = (self._signature(), str(device))
         if mode in self._packed and self._packed_sig.get(mode) == sig:
             return self._packed[mode]
@@ -416,151 +448,121 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         enc, dec = self.encoder, self.decoder
         if enc.embed_dim // enc.num_heads != 64 or dec.embed_dim // dec.num_heads != 64:
             raise NotImplementedError("fast3r_b200 attention kernel is specialised for head_dim 64")
-        pe = enc.patch_embed.proj
-        P = dict(
-            pe_w=_pk(pe.weight.detach().reshape(pe.weight.shape[0], 1, -1), x3), pe_b=_f32(pe.bias),
-            enc=[_BlockW(b, x3) for b in enc.enc_blocks], enc_nw=_f32(enc.enc_norm.weight),
-            enc_nb=_f32(enc.enc_norm.bias),
-            de_w=_w_lin(dec.decoder_embed, x3), de_b=_f32(dec.decoder_embed.bias),
-            dec=[_BlockW(b, x3) for b in dec.dec_blocks], dec_nw=_f32(dec.dec_norm.weight),
-            dec_nb=_f32(dec.dec_norm.bias),
-            table=dec.image_idx_emb.detach().to(device=device, dtype=F32).contiguous(),
-            head=_DPTW(self.downstream_head.dpt, x3),
-            head_local=_DPTW(self.downstream_head_local.dpt, x3) if self.downstream_head_local is not None else None,
-        )
-        j = torch.arange(16, dtype=torch.float32)
-        ang = torch.arange(256, dtype=torch.float32)[:, None] * (1.0 / (enc.rope_base ** (j / 16.0)))[None]
-        P["rope_cos"], P["rope_sin"] = ang.cos().contiguous().to(device), ang.sin().contiguous().to(device)
+        P = _ModelW(self, mode, device)
         self._packed[mode], self._packed_sig[mode] = P, sig
         return P
 
-    # ---- GEMM dispatch of the two numeric paths.  ``a`` is a bf16 operand (fast path) or an fp32 activation that is
-    # hi/lo-split on the fly (parity path; ``a_relu`` folds the preceding ReLU into the split).
-    @staticmethod
-    def _gemm(x3, a, wt, *, a_relu=False, a_relu_src=None, **kw):
-        if x3:
-            return ops.gemm_x3(a, wt, a_relu=a_relu, **kw)
-        return ops.gemm(a_relu_src if a_relu else a, wt, **kw)
-
-    @classmethod
-    def _linear(cls, x3, a, wt, bias=None, **kw):
-        return cls._gemm(x3, a, wt, w=a.numel() // a.shape[-1], bias=bias, **kw)
-
     # ---- one transformer block (fast3r/croco/models/blocks.py:135-194, 236-239)
-    @classmethod
-    def _block(cls, x, w: _BlockW, ws, *, batch, seq, heads, eps, scale, rope=None, kv_exchange=None, x3=False):
+    @staticmethod
+    def _block(x, w: _BlockW, ws, *, batch, seq, heads, eps, scale, rope=None, kv_exchange=None):
         M, D = x.shape
         h, q, kv, att, hid = ws["h"][:M], ws["q"][:M], ws["kv"][:M], ws["att"][:M], ws["hid"][:M]
         ops.layernorm(x, w.n1w, w.n1b, eps, h)
         if rope is not None:
-            cls._linear(x3, h, w.qkv_w, w.qkv_b, out0=q, ldo=D, split_col=D, out0b=kv, ldo_b=2 * D, epi=L.EPI_ROPE,
-                        tok_per_img=rope["P"], grid_w=rope["gw"], rope_cols=2 * D, rope_cos=rope["cos"],
-                        rope_sin=rope["sin"])
+            w.linear(h, w.qkv_w, w.qkv_b, out0=q, ldo=D, split_col=D, out0b=kv, ldo_b=2 * D, epi=L.EPI_ROPE,
+                     tok_per_img=rope["P"], grid_w=rope["gw"], rope_cols=2 * D, rope_cos=rope["cos"],
+                     rope_sin=rope["sin"])
         else:
-            cls._linear(x3, h, w.qkv_w, w.qkv_b, out0=q, ldo=D, split_col=D, out0b=kv, ldo_b=2 * D)
+            w.linear(h, w.qkv_w, w.qkv_b, out0=q, ldo=D, split_col=D, out0b=kv, ldo_b=2 * D)
         if kv_exchange is None:
-            (ops.attention_x3 if x3 else ops.attention)(q, kv, att, batch=batch, heads=heads, sq=seq, skv=seq, scale=scale)
+            (ops.attention_x3 if w.x3 else ops.attention)(q, kv, att, batch=batch, heads=heads, sq=seq, skv=seq,
+                                                          scale=scale)
         else:  # sequence parallel: exchange K|V with the other ranks and attend to all keys (parallel.KVExchange)
-            kv_exchange.attend(ops, q, kv, att, heads=heads, scale=scale, x3=x3)
-        cls._linear(x3, att, w.proj_w, w.proj_b, out0=x, res0=x)
+            kv_exchange.attend(ops, q, kv, att, heads=heads, scale=scale, x3=w.x3)
+        w.linear(att, w.proj_w, w.proj_b, out0=x, res0=x)
         ops.layernorm(x, w.n2w, w.n2b, eps, h)
-        cls._linear(x3, h, w.fc1_w, w.fc1_b, out0=hid, act=L.ACT_GELU)
-        cls._linear(x3, hid, w.fc2_w, w.fc2_b, out0=x, res0=x)
+        w.linear(h, w.fc1_w, w.fc1_b, out0=hid, act=L.ACT_GELU)
+        w.linear(hid, w.fc2_w, w.fc2_b, out0=x, res0=x)
 
     @staticmethod
-    def _workspace(M, D, hidden, device, x3=False):
-        e = lambda *s: torch.empty(*s, dtype=F32 if x3 else BF16, device=device)  # noqa: E731
+    def _workspace(M, D, hidden, device, dtype=BF16):
+        e = lambda *s: torch.empty(*s, dtype=dtype, device=device)  # noqa: E731
         return dict(h=e(M, D), q=e(M, D), kv=e(M, 2 * D), att=e(M, D), hid=e(M, hidden))
 
     # ---- encoder (fast3r/models/fast3r.py:250-296, 549-559)
-    def _encode(self, imgs: torch.Tensor, P_, x3=False):
+    def _encode(self, imgs: torch.Tensor, P_: _ModelW):
         enc = self.encoder
         n, _, H, W = imgs.shape
         gh, gw = H // enc.patch_size, W // enc.patch_size
-        if max(gh, gw) > P_["rope_cos"].shape[0]:
-            raise ValueError(f"image too large for the RoPE table ({gh}x{gw} patches > {P_['rope_cos'].shape[0]})")
+        if max(gh, gw) > P_.rope_cos.shape[0]:
+            raise ValueError(f"image too large for the RoPE table ({gh}x{gw} patches > {P_.rope_cos.shape[0]})")
         P, D = gh * gw, enc.embed_dim
-        adt = F32 if x3 else BF16
-        feats = torch.empty(n * P, D, dtype=adt, device=imgs.device)
+        feats = torch.empty(n * P, D, dtype=P_.adt, device=imgs.device)
         chunk = self.max_images_per_encoder_chunk
         hidden = enc.enc_blocks[0].mlp.fc1.weight.shape[0]
-        ws = self._workspace(min(n, chunk) * P, D, hidden, imgs.device, x3)
-        rope = dict(P=P, gw=gw, cos=P_["rope_cos"], sin=P_["rope_sin"])
+        ws = self._workspace(min(n, chunk) * P, D, hidden, imgs.device, P_.adt)
+        rope = dict(P=P, gw=gw, cos=P_.rope_cos, sin=P_.rope_sin)
         for s in range(0, n, chunk):
             c = min(chunk, n - s)
             M = c * P
-            a0 = torch.empty(M, 3 * enc.patch_size * enc.patch_size, dtype=adt, device=imgs.device)
+            a0 = torch.empty(M, 3 * enc.patch_size * enc.patch_size, dtype=P_.adt, device=imgs.device)
             ops.im2col_patch(imgs[s:s + c], a0)
             x = torch.empty(M, D, dtype=F32, device=imgs.device)
-            self._linear(x3, a0, P_["pe_w"], P_["pe_b"], out0=x)
+            P_.linear(a0, P_.pe_w, P_.pe_b, out0=x)
             self._tap("patch_embed", x)
-            if not x3 and self._taps is None and ops.pick_kv_split(attention_units(c, enc.num_heads, P), (P + 127) // 128) == 1:
+            if not P_.x3 and self._taps is None and ops.pick_kv_split(attention_units(c, enc.num_heads, P), (P + 127) // 128) == 1:
                 # all encoder blocks of this chunk in ONE library call (f3r_transformer_blocks: the same seven launches per
                 # block, issued by the C side with its own workspace carving)
-                ops.transformer_blocks(x, P_["enc"], batch=c, seq=P, heads=enc.num_heads, eps=1e-6, scale=64 ** -0.5, rope=rope)
+                ops.transformer_blocks(x, P_.enc, batch=c, seq=P, heads=enc.num_heads, eps=1e-6, scale=64 ** -0.5, rope=rope)
             else:
-                for li, w in enumerate(P_["enc"]):
-                    self._block(x, w, ws, batch=c, seq=P, heads=enc.num_heads, eps=1e-6, scale=64 ** -0.5, rope=rope, x3=x3)
+                for li, w in enumerate(P_.enc):
+                    self._block(x, w, ws, batch=c, seq=P, heads=enc.num_heads, eps=1e-6, scale=64 ** -0.5, rope=rope)
                     self._tap(f"enc_block{li}", x)
-            ops.layernorm(x, P_["enc_nw"], P_["enc_nb"], 1e-6, feats[s * P:(s + c) * P])
+            ops.layernorm(x, P_.enc_nw, P_.enc_nb, 1e-6, feats[s * P:(s + c) * P])
         return feats, P, gh, gw
 
     # ---- fusion decoder (fast3r/models/fast3r.py:768-808)
-    def _decode(self, feats_bnp: torch.Tensor, ids: torch.Tensor, B: int, n_local: int, P: int, P_, kv_exchange=None,
-                per_token_ids: bool = False, x3=False):
-        """feats_bnp: (B*seq, D) tokens in (b, view, patch) order.  ids: (B, n_local) table rows per view (P tokens
-        each), or with per_token_ids=True a flat (B*seq,) tensor with one table row per token (mixed resolutions;
-        then n_local * P must still equal the per-sample sequence length)."""
+    def _decode(self, feats_bnp: torch.Tensor, ids: torch.Tensor, B: int, seq: int, tok_per_img: int, P_: _ModelW,
+                kv_exchange=None):
+        """feats_bnp: (B*seq, D) tokens in (b, view, patch) order.  ids: image-index table rows, a (B, views) tensor
+        with one row per view of tok_per_img tokens, or with tok_per_img=0 a flat (B*seq,) tensor with one row per
+        token (views of different resolutions)."""
         dec = self.decoder
         D = dec.embed_dim
         M = feats_bnp.shape[0]
         dev = feats_bnp.device
         x = torch.empty(M, D, dtype=F32, device=dev)
-        self._linear(x3, feats_bnp, P_["de_w"], P_["de_b"], out0=x, epi=L.EPI_IDXEMB,
-                     tok_per_img=0 if per_token_ids else P, emb_table=P_["table"],
-                     emb_ids=ids.to(device=dev, dtype=torch.int32).contiguous())
+        P_.linear(feats_bnp, P_.de_w, P_.de_b, out0=x, epi=L.EPI_IDXEMB, tok_per_img=tok_per_img, emb_table=P_.table,
+                  emb_ids=ids.to(device=dev, dtype=torch.int32).contiguous())
         hd = D // dec.num_heads
         if (not self.training) and dec.attn_bias_for_inference_enabled:
             scale = hd ** -0.5 * (1.0 * math.log(137) / math.log(20)) ** 0.5  # blocks.py:119-124
         else:
             scale = hd ** -0.5
         hidden = dec.dec_blocks[0].mlp.fc1.weight.shape[0]
-        ws = self._workspace(M, D, hidden, dev, x3)
+        ws = self._workspace(M, D, hidden, dev, P_.adt)
         depth = dec.depth
         hooks = {depth * 2 // 4: None, depth * 3 // 4: None}
         self._tap("dec_embed", x)
-        for i, w in enumerate(P_["dec"]):
+        for i, w in enumerate(P_.dec):
             if kv_exchange is not None:
                 slot = kv_exchange.kv_workspace(ws["kv"].dtype, dev)
                 if slot is not None:
                     ws["kv"] = slot  # the QKV GEMM writes K|V straight into this rank's exchange slot of this layer
-            self._block(x, w, ws, batch=B, seq=n_local * P, heads=dec.num_heads, eps=1e-5, scale=scale,
-                        kv_exchange=kv_exchange, x3=x3)
+            self._block(x, w, ws, batch=B, seq=seq, heads=dec.num_heads, eps=1e-5, scale=scale, kv_exchange=kv_exchange)
             self._tap(f"dec_block{i}", x)
             if (i + 1) in hooks:
-                if x3:
+                if P_.x3:
                     hooks[i + 1] = x.clone()
                 else:
                     t = torch.empty(M, D, dtype=BF16, device=dev)
                     ops.cast_bf16(x, t)
                     hooks[i + 1] = t
-        last = torch.empty(M, D, dtype=F32 if x3 else BF16, device=dev)
-        ops.layernorm(x, P_["dec_nw"], P_["dec_nb"], 1e-6, last)
+        last = torch.empty(M, D, dtype=P_.adt, device=dev)
+        ops.layernorm(x, P_.dec_nw, P_.dec_nb, 1e-6, last)
         return [hooks[depth * 2 // 4], hooks[depth * 3 // 4], last]
 
     # ---- DPT head + postprocess (dpt_head.py:42-90, dpt_block.py, postprocess.py)
-    @classmethod
-    def _rcu(cls, x, x_relu, w, nv, h, w_, res1=None, want_relu=False, x3=False):
+    @staticmethod
+    def _rcu(hw: _DPTW, x, x_relu, w, nv, h, w_, res1=None, want_relu=False):
         """y = x + conv2(relu(conv1(relu(x)))) (+ res1); returns (y, relu(y) or None).  Fast path: relu(x) arrives as
         the bf16 tensor x_relu and relu(y) is a second epilogue output; parity path: the ReLUs are folded into the
         operand split of the consuming conv (x_relu / the returned relu(y) are None)."""
         dev = x.device
-        adt = F32 if x3 else BF16
-        t = torch.empty(nv, h, w_, 256, dtype=adt, device=dev)
-        cls._gemm(x3, x, w[0], a_relu=True, a_relu_src=x_relu, w=w_, h=h, nb=nv, taps=9, bias=w[1], out0=t,
-                  act=L.ACT_RELU)
-        y = torch.empty(nv, h, w_, 256, dtype=adt, device=dev)
-        if x3:
+        t = torch.empty(nv, h, w_, 256, dtype=hw.adt, device=dev)
+        hw.gemm(x, w[0], a_relu=True, a_relu_src=x_relu, w=w_, h=h, nb=nv, taps=9, bias=w[1], out0=t, act=L.ACT_RELU)
+        y = torch.empty(nv, h, w_, 256, dtype=hw.adt, device=dev)
+        if hw.x3:
             ops.gemm_x3(t, w[2], w=w_, h=h, nb=nv, taps=9, bias=w[3], out0=y, res0=x)
             if res1 is not None:
                 ops.add_f32(y, res1)
@@ -570,11 +572,10 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         return y, yr
 
     def _dpt(self, hooked: List[torch.Tensor], nv: int, gh: int, gw: int, H: int, W: int, hw: _DPTW,
-             pts: torch.Tensor, conf: torch.Tensor, x3=False):
+             pts: torch.Tensor, conf: torch.Tensor):
         dev = hooked[0].device
-        adt = F32 if x3 else BF16
-        e = lambda *s: torch.empty(*s, dtype=adt, device=dev)  # noqa: E731
-        g = lambda a, wt, **kw: self._gemm(x3, a, wt, **kw)  # noqa: E731
+        e = lambda *s: torch.empty(*s, dtype=hw.adt, device=dev)  # noqa: E731
+        g = hw.gemm
         # act_postprocess
         a = e(nv, gh, gw, 96)
         g(hooked[0], hw.ap0[0], w=gw, h=gh, nb=nv, bias=hw.ap0[1], out0=a)
@@ -590,7 +591,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         g(hooked[3], hw.ap3[0], w=gw, h=gh, nb=nv, bias=hw.ap3[1], out0=a)
         h3, w3 = (gh + 1) // 2, (gw + 1) // 2
         l3 = e(nv, h3, w3, 768)
-        if x3:  # stride-2 conv = strided im2col of the split operand (channels [hi | lo | hi]) + linear
+        if hw.x3:  # stride-2 conv = strided im2col of the split operand (channels [hi | lo | hi]) + linear
             a3 = torch.empty(nv, gh, gw, 3 * 768, dtype=BF16, device=dev)
             ops.split3(a, a3)
             col = torch.empty(nv * h3 * w3, 27 * 768, dtype=BF16, device=dev)
@@ -605,7 +606,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         for i, src in enumerate([l0, l1, l2, l3]):
             hh, ww = dims[i]
             o = e(nv, hh, ww, 256)
-            orl = None if x3 else e(nv, hh, ww, 256)
+            orl = None if hw.x3 else e(nv, hh, ww, 256)
             g(src, hw.rn[i], w=ww, h=hh, nb=nv, taps=9, out0=o, out1=orl)
             lay.append(o)
             lay_r.append(orl)
@@ -620,14 +621,14 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
             return up
 
         # refinenet4 (single input; output cropped to layer-3 size, dpt_head.py:69-71)
-        y, _ = self._rcu(lay[3], lay_r[3], hw.fus[4]["r2"], nv, h3, w3, x3=x3)
+        y, _ = self._rcu(hw, lay[3], lay_r[3], hw.fus[4]["r2"], nv, h3, w3)
         path = out_conv_up(y, hw.fus[4], h3, w3, gh, gw)
         self._tap("path4", path)
         for lvl, i in ((3, 2), (2, 1), (1, 0)):
             hh, ww = dims[i]
             f = hw.fus[lvl]
-            s, sr = self._rcu(lay[i], lay_r[i], f["r1"], nv, hh, ww, res1=path, want_relu=True, x3=x3)
-            y, _ = self._rcu(s, sr, f["r2"], nv, hh, ww, x3=x3)
+            s, sr = self._rcu(hw, lay[i], lay_r[i], f["r1"], nv, hh, ww, res1=path, want_relu=True)
+            y, _ = self._rcu(hw, s, sr, f["r2"], nv, hh, ww)
             path = out_conv_up(y, f, hh, ww, 2 * hh, 2 * ww)
             self._tap(f"path{lvl}", path)
         # head: conv3x3 256->128, x2 bilinear, conv3x3 128->128 + ReLU + conv1x1 128->4 + postprocess (fused)
@@ -638,22 +639,22 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         ops.upsample2x(t, up, nv, hh, ww, 128, H, W)
         g(up, hw.h2[0], w=W, h=H, nb=nv, taps=9, bias=hw.h2[1], epi=L.EPI_FINAL, w4=hw.w4, b4=hw.b4, pts=pts, conf=conf)
 
-    def _run_heads(self, hooked, nvt, P, gh, gw, H, W, P_, device, x3):
+    def _run_heads(self, hooked, nvt, P, gh, gw, H, W, P_: _ModelW, device):
         """All views of one resolution through the global (and local) DPT head in chunks of
         max_parallel_views_for_head (fast3r.py:430-444).  Returns {"pts", "conf"[, "pts_local", "conf_local"]}."""
-        heads = [("", P_["head"])] + ([("_local", P_["head_local"])] if P_["head_local"] is not None else [])
+        heads = [("", P_.head)] + ([("_local", P_.head_local)] if P_.head_local is not None else [])
         outs = {}
         for suffix, _hw in heads:
             outs["pts" + suffix] = torch.empty(nvt, H, W, 3, dtype=F32, device=device)
             outs["conf" + suffix] = torch.empty(nvt, H, W, dtype=F32, device=device)
         step = max(1, int(self.max_parallel_views_for_head))
-        if x3:
+        if P_.x3:
             step = min(step, 8)  # fp32 feature maps + split scratch are ~5x the bf16 footprint
         for s in range(0, nvt, step):
             c = min(step, nvt - s)
             hk = [t[s * P:(s + c) * P] for t in hooked]
             for suffix, hw in heads:
-                self._dpt(hk, c, gh, gw, H, W, hw, outs["pts" + suffix][s:s + c], outs["conf" + suffix][s:s + c], x3=x3)
+                self._dpt(hk, c, gh, gw, H, W, hw, outs["pts" + suffix][s:s + c], outs["conf" + suffix][s:s + c])
             if self._host_sink is not None:  # D2H of this chunk overlaps the heads of the next one (SURVEY §8 f1)
                 self._host_sink.chunk_done(list(outs.values()), s, c)
         return outs
@@ -665,88 +666,6 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         if "pts_local" in outs:
             r["pts3d_local"] = outs["pts_local"][j * B:(j + 1) * B]
             r["conf_local"] = outs["conf_local"][j * B:(j + 1) * B]
-
-    # ---- views of different resolutions (fast3r/models/fast3r.py:276-294, 364-376, 407-428)
-    def _forward_mixed(self, views, profiling=False):
-        """The reference encodes and decodes heads view by view when resolutions differ; here views are grouped by
-        shape (same arithmetic per view, batched per group), the fusion decoder runs once over the concatenation of
-        all tokens in view order with one image-index-embedding row per token."""
-        if self.sp_group is not None:
-            raise NotImplementedError("fast3r_b200: sequence parallel needs views of one resolution")
-        profiling_info = {} if profiling else None
-        t_start = time.time()
-        device = views[0]["img"].device
-        x3 = self.precision == "fp32"
-        P_ = self._pack(device, x3)
-        N = len(views)
-        B = views[0]["img"].shape[0]
-        ps = self.encoder.patch_size
-        groups: Dict[tuple, List[int]] = {}
-        for i, v in enumerate(views):
-            b, _, H, W = v["img"].shape
-            if b != B:
-                raise ValueError("all views must have the same batch size")
-            if H % ps or W % ps:
-                raise AssertionError(f"Input image size ({H}x{W}) is not a multiple of patch size ({ps}).")
-            groups.setdefault((H, W), []).append(i)
-        D = self.encoder.embed_dim
-        tok = [0] * N            # tokens per view
-        genc = {}
-        for (H, W), idxs in groups.items():
-            imgs = torch.cat([views[i]["img"] for i in idxs], dim=0).to(dtype=F32).contiguous()
-            feats, P, gh, gw = self._encode(imgs, P_, x3)  # ((n_g*B)*P, D) in (n, b, p) order
-            genc[(H, W)] = (feats, P, gh, gw)
-            for i in idxs:
-                tok[i] = P
-        if profiling:
-            _sync(device)
-            profiling_info["encode_images_time"] = time.time() - t_start
-        t1 = time.time()
-        ids = self.decoder.draw_image_ids(B, N, rank_offset=self.image_id_rank_offset)
-        off = [0]
-        for i in range(N):
-            off.append(off[-1] + tok[i])
-        S = off[-1]
-        if profiling:
-            profiling_info["pos_emb_time"] = time.time() - t1
-            _sync(device)
-        t2 = time.time()
-        # (b, view, patch) row of every encoder token: one index_copy per resolution group instead of per-view slices
-        adt = F32 if x3 else BF16
-        feats_bnp = torch.empty(B * S, D, dtype=adt, device=device)
-        tok_ids = torch.empty(B, S, dtype=torch.int32)
-        rows = {}
-        for (H, W), idxs in groups.items():
-            feats, P, _, _ = genc[(H, W)]
-            base = torch.tensor([off[i] for i in idxs], dtype=torch.long)  # (n_g,)
-            r = (base[:, None, None] + torch.arange(B, dtype=torch.long)[None, :, None] * S
-                 + torch.arange(P, dtype=torch.long)[None, None, :]).reshape(-1).to(device)  # (n_g, B, P) order
-            rows[(H, W)] = r
-            feats_bnp.index_copy_(0, r, feats)
-            for i in idxs:
-                tok_ids[:, off[i]: off[i] + P] = ids[:, i:i + 1].to(torch.int32)
-        h12, h18, h24 = self._decode(feats_bnp, tok_ids.reshape(-1), B, 1, S, P_, per_token_ids=True, x3=x3)
-        if profiling:
-            _sync(device)
-            profiling_info["decoder_time"] = time.time() - t2
-        t3 = time.time()
-        final_results = [{} for _ in range(N)]
-        t4 = time.time()
-        for (H, W), idxs in groups.items():
-            feats, P, gh, gw = genc[(H, W)]
-            r = rows[(H, W)]
-            hooked = [feats, h12.index_select(0, r), h18.index_select(0, r), h24.index_select(0, r)]  # '(n b) p'
-            outs = self._run_heads(hooked, len(idxs) * B, P, gh, gw, H, W, P_, device, x3)
-            for k, i in enumerate(idxs):
-                self._fill_result(final_results[i], outs, k, B)
-        if profiling:
-            _sync(device)
-            t_end = time.time()
-            profiling_info["head_prepare_input_time"] = t4 - t3
-            profiling_info["head_forward_time"] = t_end - t4
-            profiling_info["total_time"] = t_end - t_start
-            return final_results, profiling_info
-        return final_results
 
     # ---- portrait views (ManyAR_PatchEmbed + landscape_only heads: fast3r/dust3r/patch_embed.py:59-105,
     #      fast3r/dust3r/utils/misc.py:74-104)
@@ -777,24 +696,6 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
                                           "all batch elements of a view")
         return flags
 
-    def _forward_portrait(self, views, portrait, profiling):
-        """Portrait views are un-transposed (a strided view of the same pixels), go through the shape-grouped path in their
-        true geometry - patch grid, RoPE positions and DPT head at (W, H) - and their predictions are transposed back to
-        the landscape storage layout, exactly what ManyAR_PatchEmbed + transpose_to_landscape.wrapper_yes compute."""
-        vs = []
-        for v, p in zip(views, portrait):
-            if p:
-                v = dict(v)
-                v["img"] = v["img"].swapaxes(-1, -2)
-            vs.append(v)
-        out = self._forward_mixed(vs, profiling)
-        res, info = out if profiling else (out, None)
-        for r, p in zip(res, portrait):
-            if p:
-                for k in list(r):
-                    r[k] = r[k].swapaxes(1, 2)
-        return (res, info) if profiling else res
-
     # ---- forward (fast3r/models/fast3r.py:302-497)
     def forward(self, views, profiling=False):
         if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
@@ -811,32 +712,40 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         # scale 1/8, fast3r/croco/models/blocks.py:151-154 - are honoured and tested; optimisation steps are not.)
         profiling_info = {} if profiling else None
         t_start = time.time()
-        same_shape = all(v["img"].shape == views[0]["img"].shape for v in views)
-        if not same_shape:
-            return self._forward_mixed(views, profiling)
-        device = views[0]["img"].device
-        if self.sp_group is not None and device.type != "cuda":
-            device = next(self.parameters()).device  # sharded forward: host views are uploaded per rank below
-        x3 = self.precision == "fp32"
-        P_ = self._pack(device, x3)
         N = len(views)
         B, _, H, W = views[0]["img"].shape
         ps = self.encoder.patch_size
-        if H % ps or W % ps:
-            raise AssertionError(f"Input image size ({H}x{W}) is not a multiple of patch size ({ps}).")
-        portrait = self._portrait_flags(views, H, W)
-        if any(portrait):
-            return self._forward_portrait(views, portrait, profiling)
+        for v in views:
+            b, _, h, w = v["img"].shape
+            if b != B:
+                raise ValueError("all views must have the same batch size")
+            if h % ps or w % ps:
+                raise AssertionError(f"Input image size ({h}x{w}) is not a multiple of patch size ({ps}).")
+        # Portrait views (ManyAR_PatchEmbed + landscape_only heads) are recognised when all views share one stored
+        # shape.  They are un-transposed (a strided view of the same pixels) and run in their true geometry - patch grid,
+        # RoPE positions and DPT head at (W, H); their predictions are transposed back to the landscape storage layout
+        # below, exactly what ManyAR_PatchEmbed + transpose_to_landscape.wrapper_yes compute.
+        same_shape = all(v["img"].shape == views[0]["img"].shape for v in views)
+        portrait = self._portrait_flags(views, H, W) if same_shape else [False] * N
+        imgs = [v["img"].swapaxes(-1, -2) if p else v["img"] for v, p in zip(views, portrait)]
+        # Views of different resolutions (fast3r/models/fast3r.py:276-294, 364-376, 407-428): the reference encodes them
+        # and runs the heads view by view; here views are grouped by shape (same arithmetic per view, batched per group).
+        groups: Dict[tuple, List[int]] = {}
+        for i, im in enumerate(imgs):
+            groups.setdefault(tuple(im.shape[-2:]), []).append(i)
         sp = self.sp_group
-        if sp is None:
-            lo, hi = 0, N
-        else:
-            lo, hi = sp.view_range(N)
-        n_loc = hi - lo
-        imgs = torch.cat([views[i]["img"].to(device, non_blocking=True) for i in range(lo, hi)],
-                         dim=0).to(dtype=F32).contiguous()  # (n_loc*B, 3, H, W)
-
-        feats, P, gh, gw = self._encode(imgs, P_, x3)  # (n_loc*B*P, D), order (n, b, p)
+        if sp is not None and len(groups) > 1:
+            raise NotImplementedError("fast3r_b200: sequence parallel needs views of one resolution")
+        device = views[0]["img"].device
+        if sp is not None and device.type != "cuda":
+            device = next(self.parameters()).device  # sharded forward: host views are uploaded per rank below
+        P_ = self._pack(device)
+        lo, hi = (0, N) if sp is None else sp.view_range(N)
+        enc = []  # per group: ((H, W), this rank's views, their encoder tokens in (view, b, patch) order, P, gh, gw)
+        for shape, idxs in groups.items():
+            idxs = [i for i in idxs if lo <= i < hi]
+            x = torch.cat([imgs[i].to(device, non_blocking=True) for i in idxs], dim=0).to(dtype=F32).contiguous()
+            enc.append((shape, idxs) + self._encode(x, P_))
         if profiling:
             _sync(device)
             profiling_info["encode_images_time"] = time.time() - t_start
@@ -851,31 +760,55 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
             profiling_info["pos_emb_time"] = time.time() - t1
             _sync(device)
         t2 = time.time()
-        D = self.encoder.embed_dim
-        if B == 1:
-            feats_bnp = feats
-        else:  # (n, b, p) -> (b, n, p)
-            feats_bnp = feats.view(n_loc, B, P, D).permute(1, 0, 2, 3).contiguous().view(-1, D)
-        ids_loc = ids[:, lo:hi].contiguous()
-        kvx = sp.make_kv_exchange(B, n_loc * P, self.decoder.embed_dim) if sp is not None else None
-        h12, h18, h24 = self._decode(feats_bnp, ids_loc, B, n_loc, P, P_, kv_exchange=kvx, x3=x3)
+        # decoder input: the tokens of each sample in (view, patch) order; to_heads[g] takes a decoder output back to
+        # group g's (view, b, patch) order, the order of the head input (fast3r.py:385-398)
+        if len(enc) == 1:  # one image id per view
+            (_, idxs, feats, P, _, _), = enc
+            seq, tok_per_img, ids = len(idxs) * P, P, ids[:, lo:hi].contiguous()
+            if B == 1:
+                feats_bnp, to_heads = feats, [lambda t: t]
+            else:  # (n, b, p) <-> (b, n, p)
+                n = len(idxs)
+                swap = lambda t, a, b: t.view(a, b, P, -1).permute(1, 0, 2, 3).contiguous().view(a * b * P, -1)  # noqa: E731
+                feats_bnp, to_heads = swap(feats, n, B), [lambda t: swap(t, B, n)]
+        else:  # one image-index row per token; one index_copy / index_select per group instead of per-view slices
+            tok = [0] * N
+            for _, idxs, _, P, _, _ in enc:
+                for i in idxs:
+                    tok[i] = P
+            off = list(accumulate(tok, initial=0))
+            seq, tok_per_img = off[-1], 0
+            feats_bnp = torch.empty(B * seq, self.encoder.embed_dim, dtype=P_.adt, device=device)
+            tok_ids = torch.empty(B, seq, dtype=torch.int32)
+            to_heads = []
+            for _, idxs, feats, P, _, _ in enc:
+                base = torch.tensor([off[i] for i in idxs], dtype=torch.long)  # (n_g,)
+                r = (base[:, None, None] + torch.arange(B, dtype=torch.long)[None, :, None] * seq
+                     + torch.arange(P, dtype=torch.long)[None, None, :]).reshape(-1).to(device)  # (n_g, B, P) order
+                feats_bnp.index_copy_(0, r, feats)
+                for i in idxs:
+                    tok_ids[:, off[i]: off[i] + P] = ids[:, i:i + 1].to(torch.int32)
+                to_heads.append(lambda t, r=r: t.index_select(0, r))
+            ids = tok_ids.reshape(-1)
+        kvx = sp.make_kv_exchange(B, seq, self.decoder.embed_dim) if sp is not None else None
+        dec_out = self._decode(feats_bnp, ids, B, seq, tok_per_img, P_, kv_exchange=kvx)
         if profiling:
             _sync(device)
             profiling_info["decoder_time"] = time.time() - t2
         t3 = time.time()
-        Dd = self.decoder.embed_dim
-        if B == 1:
-            hooked = [feats, h12, h18, h24]
-        else:  # 'B (n p) D -> (n B) p D'  (fast3r.py:385-398)
-            back = lambda t: t.view(B, n_loc, P, Dd).permute(1, 0, 2, 3).contiguous().view(-1, Dd)  # noqa: E731
-            hooked = [feats, back(h12), back(h18), back(h24)]
+        hooked = [[feats] + [to_head(t) for t in dec_out] for (_, _, feats, _, _, _), to_head in zip(enc, to_heads)]
         if profiling:
             profiling_info["head_prepare_input_time"] = time.time() - t3
         t4 = time.time()
-        outs = self._run_heads(hooked, n_loc * B, P, gh, gw, H, W, P_, device, x3)
         final_results = [{} for _ in range(N)]
-        for i in range(lo, hi):
-            self._fill_result(final_results[i], outs, i - lo, B)
+        for ((H, W), idxs, _, P, gh, gw), hk in zip(enc, hooked):
+            outs = self._run_heads(hk, len(idxs) * B, P, gh, gw, H, W, P_, device)
+            for k, i in enumerate(idxs):
+                self._fill_result(final_results[i], outs, k, B)
+        for r, p in zip(final_results, portrait):
+            if p:
+                for k in list(r):
+                    r[k] = r[k].swapaxes(1, 2)
         if sp is not None and sp.gather_preds:
             final_results = sp.gather_results(final_results, N, B, H, W, device)
         if profiling:
