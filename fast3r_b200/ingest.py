@@ -17,7 +17,7 @@ from typing import Dict, Tuple
 import numpy as np
 import torch
 
-from . import lib as L
+from . import lib as L, ops
 
 BICUBIC, LANCZOS = 0, 1
 _TABLES: Dict[Tuple, Tuple] = {}
@@ -84,11 +84,9 @@ def ingest_rgb8(img_u8: torch.Tensor, size: int = 512, square_ok: bool = False, 
         tmp = torch.empty(h1, nw, 3, dtype=torch.uint8, device=dev)
     if nh != h1:
         vb, vk, vks, _ = _tables(h1, nh, filt, dev)
-    p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-    with torch.cuda.device(dev):
-        L.check(L.load().f3r_ingest_rgb8(p(img_u8), h1, w1, nh, nw, p(hb), p(hk), hks, span, p(vb), p(vk), vks, p(tmp),
-                                         left, top, cw, ch, p(out), torch.cuda.current_stream(dev).cuda_stream),
-                "f3r_ingest_rgb8")
+    p = ops._ptr
+    ops._call("f3r_ingest_rgb8", img_u8, p(img_u8), h1, w1, nh, nw, p(hb), p(hk), hks, span, p(vb), p(vk), vks, p(tmp),
+              left, top, cw, ch, p(out))
     return out, (ch, cw)
 
 

@@ -42,12 +42,45 @@ class BlockWeights(C.Structure):
                                           "fc1_w", "fc1_b", "fc2_w", "fc2_b")]
 
 
-EXPORTS = ["f3r_last_error", "f3r_abi_version", "f3r_gemm_desc_size", "f3r_launch_count", "f3r_gemm", "f3r_attention",
-           "f3r_layernorm", "f3r_im2col_patch", "f3r_im2col3x3s2", "f3r_upsample2x", "f3r_cast_bf16", "f3r_split3",
-           "f3r_add_f32", "f3r_attention_x3_workspace", "f3r_attention_x3", "f3r_set_option", "f3r_attention_partial",
-           "f3r_attention_merge", "f3r_resample_ksize", "f3r_resample_coeffs", "f3r_ingest_rgb8",
-           "f3r_transformer_workspace", "f3r_transformer_blocks", "f3r_conf_quantile", "f3r_similarity_fit_workspace",
-           "f3r_similarity_fit", "f3r_similarity_apply", "f3r_focal_workspace", "f3r_focal_weiszfeld"]
+# name -> (restype, argtypes), one entry per prototype of include/fast3r_b200.h, in header order.  ctypes does not check
+# these against the C side: tests/test_cabi_bindings_cpu.py compares every entry with the header.  Device pointers and
+# the cudaStream_t are void*.
+_P, _I32, _F32, _SIZE = C.c_void_p, C.c_int32, C.c_float, C.c_size_t
+_API = {
+    "f3r_last_error": (C.c_char_p, []),
+    "f3r_abi_version": (C.c_int, []),
+    "f3r_gemm_desc_size": (_SIZE, []),
+    "f3r_launch_count": (C.c_uint64, []),
+    "f3r_set_option": (C.c_int, [C.c_char_p, _I32]),
+    "f3r_gemm": (C.c_int, [C.POINTER(GemmDesc), _P]),
+    "f3r_attention": (C.c_int, [_P, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _F32, _P]),
+    "f3r_attention_partial": (C.c_int, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _P, _P, _I32, _I32, _I32, _I32,
+                                        _F32, _P]),
+    "f3r_attention_merge": (C.c_int, [_P, _P, _I32, _P, _I32, _I32, _I32, _I32, _P]),
+    "f3r_layernorm": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _F32, _P]),
+    "f3r_im2col_patch": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _P]),
+    "f3r_im2col3x3s2": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
+    "f3r_upsample2x": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
+    "f3r_cast_bf16": (C.c_int, [_P, _P, _SIZE, _P]),
+    "f3r_transformer_workspace": (_SIZE, [_I32, _I32, _I32]),
+    "f3r_transformer_blocks": (C.c_int, [C.POINTER(BlockWeights), _I32, _P, _I32, _I32, _I32, _I32, _I32, _F32, _F32,
+                                         _I32, _I32, _P, _P, _P, _SIZE, _P]),
+    "f3r_resample_ksize": (C.c_int, [_I32, _I32, _I32]),
+    "f3r_resample_coeffs": (C.c_int, [_I32, _I32, _I32, _P, _P]),
+    "f3r_ingest_rgb8": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _I32, _I32, _P, _P, _I32, _P, _I32, _I32, _I32,
+                                  _I32, _P, _P]),
+    "f3r_conf_quantile": (C.c_int, [_P, _I32, _I32, _F32, _P, _P]),
+    "f3r_similarity_fit_workspace": (_SIZE, [_I32]),
+    "f3r_similarity_fit": (C.c_int, [_P, _P, _P, _P, _P, _I32, _I32, _P, _P, _SIZE, _P]),
+    "f3r_similarity_apply": (C.c_int, [_P, _P, _P, _I32, _I32, _P]),
+    "f3r_focal_workspace": (_SIZE, [_I32]),
+    "f3r_focal_weiszfeld": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _SIZE, _P]),
+    "f3r_split3": (C.c_int, [_P, _P, _SIZE, _I32, _I32, _P]),
+    "f3r_add_f32": (C.c_int, [_P, _P, _SIZE, _P]),
+    "f3r_attention_x3_workspace": (_SIZE, [_I32, _I32, _I32, _I32]),
+    "f3r_attention_x3": (C.c_int, [_P, _I32, _P, _I32, _P, _I32, _P, _P, _SIZE, _I32, _I32, _I32, _I32, _F32, _P]),
+}
+EXPORTS = list(_API)
 
 _lib = None
 
@@ -62,66 +95,9 @@ def load() -> C.CDLL:
             f"{LIB_PATH} not found: build it with `python -m fast3r_b200.build` (or __graft_entry__.build()). "
             "fast3r_b200 has no CPU / PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
-    lib.f3r_last_error.restype = C.c_char_p
-    lib.f3r_abi_version.restype = C.c_int
-    lib.f3r_launch_count.restype = C.c_uint64
-    lib.f3r_gemm.argtypes = [C.POINTER(GemmDesc), C.c_void_p]
-    lib.f3r_attention_partial.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                          C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                          C.c_float, C.c_void_p]
-    lib.f3r_attention_merge.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                        C.c_int32, C.c_void_p]
-    lib.f3r_attention_partial.restype = C.c_int
-    lib.f3r_attention_merge.restype = C.c_int
-    lib.f3r_resample_ksize.argtypes = [C.c_int32, C.c_int32, C.c_int32]
-    lib.f3r_resample_ksize.restype = C.c_int
-    lib.f3r_resample_coeffs.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-    lib.f3r_resample_coeffs.restype = C.c_int
-    lib.f3r_ingest_rgb8.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
-                                    C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
-                                    C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]
-    lib.f3r_ingest_rgb8.restype = C.c_int
-    lib.f3r_transformer_workspace.argtypes = [C.c_int32, C.c_int32, C.c_int32]
-    lib.f3r_transformer_workspace.restype = C.c_size_t
-    lib.f3r_transformer_blocks.argtypes = [C.POINTER(BlockWeights), C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                           C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_int32, C.c_void_p,
-                                           C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.f3r_transformer_blocks.restype = C.c_int
-    lib.f3r_conf_quantile.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p]
-    lib.f3r_similarity_fit_workspace.argtypes = [C.c_int32]
-    lib.f3r_similarity_fit_workspace.restype = C.c_size_t
-    lib.f3r_similarity_fit.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
-                                       C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.f3r_similarity_apply.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
-    lib.f3r_focal_workspace.argtypes = [C.c_int32]
-    lib.f3r_focal_workspace.restype = C.c_size_t
-    lib.f3r_focal_weiszfeld.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                        C.c_int32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    for name in ("f3r_conf_quantile", "f3r_similarity_fit", "f3r_similarity_apply", "f3r_focal_weiszfeld"):
-        getattr(lib, name).restype = C.c_int
-    lib.f3r_set_option.argtypes = [C.c_char_p, C.c_int32]
-    lib.f3r_set_option.restype = C.c_int
-    lib.f3r_attention.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
-                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p]
-    lib.f3r_layernorm.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                  C.c_float, C.c_void_p]
-    lib.f3r_im2col_patch.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
-    lib.f3r_im2col3x3s2.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                    C.c_int32, C.c_void_p]
-    lib.f3r_upsample2x.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                   C.c_int32, C.c_int32, C.c_void_p]
-    lib.f3r_split3.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int32, C.c_int32, C.c_void_p]
-    lib.f3r_add_f32.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.f3r_attention_x3_workspace.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
-    lib.f3r_attention_x3_workspace.restype = C.c_size_t
-    lib.f3r_attention_x3.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
-                                     C.c_void_p, C.c_size_t, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
-                                     C.c_void_p]
-    lib.f3r_cast_bf16.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    for name in ("f3r_gemm", "f3r_attention", "f3r_layernorm", "f3r_im2col_patch", "f3r_im2col3x3s2",
-                 "f3r_upsample2x", "f3r_cast_bf16", "f3r_split3", "f3r_add_f32", "f3r_attention_x3"):
-        getattr(lib, name).restype = C.c_int
-    lib.f3r_gemm_desc_size.restype = C.c_size_t
+    for name, (restype, argtypes) in _API.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if lib.f3r_abi_version() != ABI_VERSION or lib.f3r_gemm_desc_size() != C.sizeof(GemmDesc):
         raise RuntimeError("libfast3r_b200.so ABI mismatch (rebuild: python -m fast3r_b200.build --force)")
     _lib = lib

@@ -17,27 +17,26 @@ BF16, F32 = torch.bfloat16, torch.float32
 KERNEL_TIMER = None
 
 
-def _stream(t: Optional[torch.Tensor] = None) -> int:
-    """The current stream OF THE TENSOR'S DEVICE (callers need not have made that device current)."""
-    return torch.cuda.current_stream(t.device if t is not None else None).cuda_stream
+def _call(name: str, anchor: torch.Tensor, *args) -> None:
+    """Calls library entry point `name` with `args` followed by the current stream of the CUDA tensor `anchor`'s device,
+    and raises if it fails.  CUDA runtime calls inside the library (cudaFuncSetAttribute, launches) act on the CURRENT
+    device, so the anchor's device is made current for the duration of the call (callers need not have done so)."""
+    idx = anchor.device.index
+    prev = torch.cuda.current_device()
+    if prev != idx:
+        torch.cuda.set_device(idx)
+    try:
+        rc = getattr(L.load(), name)(*args, torch.cuda.current_stream(idx).cuda_stream)
+    finally:
+        if prev != idx:
+            torch.cuda.set_device(prev)
+    L.check(rc, name)
 
 
-class _on_device:
-    """CUDA runtime calls inside the library (cudaFuncSetAttribute, launches) act on the CURRENT device: make the
-    operand's device current for the duration of the call."""
-
-    def __init__(self, t: torch.Tensor):
-        self.idx = t.device.index if t.is_cuda else None
-
-    def __enter__(self):
-        self.prev = None
-        if self.idx is not None and torch.cuda.current_device() != self.idx:
-            self.prev = torch.cuda.current_device()
-            torch.cuda.set_device(self.idx)
-
-    def __exit__(self, *exc):
-        if self.prev is not None:
-            torch.cuda.set_device(self.prev)
+def _scratch(nbytes: int, device) -> torch.Tensor:
+    """Device workspace for one call.  The caching allocator aligns every block to >= 512 bytes, which covers the
+    256-byte and 8-byte alignment the library's workspace arguments require."""
+    return torch.empty(nbytes, dtype=torch.uint8, device=device)
 
 
 def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
@@ -101,8 +100,7 @@ def gemm(a: torch.Tensor, wt: torch.Tensor, *, w: int, h: int = 1, nb: int = 1, 
     d.rope_cos, d.rope_sin = _ptr(rope_cos), _ptr(rope_sin)
     d.emb_table, d.emb_ids = _ptr(emb_table), _ptr(emb_ids)
     d.w4, d.b4, d.pts, d.conf = _ptr(w4), _ptr(b4), _ptr(pts), _ptr(conf)
-    with _on_device(a):
-        L.check(L.load().f3r_gemm(C.byref(d), _stream(a)), "f3r_gemm")
+    _call("f3r_gemm", a, C.byref(d))
 
 
 def gemm_x3(a: torch.Tensor, wt3: torch.Tensor, *, a_relu: bool = False, **kw):
@@ -120,15 +118,13 @@ def split3(x: torch.Tensor, out: torch.Tensor, relu: bool = False):
     _chk(x, F32, "x"); _chk(out, BF16, "out")
     k = x.shape[-1]
     assert out.numel() == 3 * x.numel()
-    with _on_device(x):
-        L.check(L.load().f3r_split3(_ptr(x), _ptr(out), x.numel() // k, k, int(relu), _stream(x)), "f3r_split3")
+    _call("f3r_split3", x, _ptr(x), _ptr(out), x.numel() // k, k, int(relu))
 
 
 def add_f32(dst: torch.Tensor, src: torch.Tensor):
     _chk(dst, F32, "dst"); _chk(src, F32, "src")
     assert dst.numel() == src.numel()
-    with _on_device(dst):
-        L.check(L.load().f3r_add_f32(_ptr(dst), _ptr(src), dst.numel(), _stream(dst)), "f3r_add_f32")
+    _call("f3r_add_f32", dst, _ptr(dst), _ptr(src), dst.numel())
 
 
 def linear(a: torch.Tensor, wt: torch.Tensor, bias=None, **kw):
@@ -172,19 +168,15 @@ def attention_partial(q: torch.Tensor, kv: torch.Tensor, part_o: torch.Tensor, p
     slots = part_o.shape[0]
     assert part_base + n_split <= slots and part_o.numel() == slots * batch * sq * heads * 64
     assert part_lse.numel() == slots * batch * heads * sq
-    with _on_device(q):
-        L.check(L.load().f3r_attention_partial(_ptr(q), ldq, _ptr(kv), ldkv, kv_rows_total, kv_row0, skv, n_split,
-                                               _ptr(part_o), _ptr(part_lse), part_base, batch, heads, sq, float(scale),
-                                               _stream(q)), "f3r_attention_partial")
+    _call("f3r_attention_partial", q, _ptr(q), ldq, _ptr(kv), ldkv, kv_rows_total, kv_row0, skv, n_split, _ptr(part_o),
+          _ptr(part_lse), part_base, batch, heads, sq, float(scale))
 
 
 def attention_merge(part_o: torch.Tensor, part_lse: torch.Tensor, n_parts: int, out: torch.Tensor, *, batch: int,
                     heads: int, sq: int):
     _chk(part_o, F32, "part_o"); _chk(part_lse, F32, "part_lse"); _chk(out, BF16, "out")
     assert out.numel() == batch * sq * out.shape[-1] and n_parts <= part_o.shape[0]
-    with _on_device(out):
-        L.check(L.load().f3r_attention_merge(_ptr(part_o), _ptr(part_lse), n_parts, _ptr(out), out.shape[-1], batch,
-                                             heads, sq, _stream(out)), "f3r_attention_merge")
+    _call("f3r_attention_merge", out, _ptr(part_o), _ptr(part_lse), n_parts, _ptr(out), out.shape[-1], batch, heads, sq)
 
 
 def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: int, heads: int, sq: int, skv: int,
@@ -195,8 +187,8 @@ def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: in
     ldq, ldkv, ldo = q.shape[-1], kv.shape[-1], out.shape[-1]
     assert q.numel() == batch * sq * ldq and kv.numel() == batch * skv * ldkv and out.numel() == batch * sq * ldo
     timer = KERNEL_TIMER
-    st = torch.cuda.current_stream(q.device)
     if timer is not None:
+        st = torch.cuda.current_stream(q.device)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(st)
     ns = kv_split if kv_split is not None else (
@@ -208,9 +200,8 @@ def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: in
                           kv_rows_total=skv, kv_row0=0, skv=skv, scale=scale)
         attention_merge(part_o, part_lse, ns, out, batch=batch, heads=heads, sq=sq)
     else:
-        with _on_device(q):
-            L.check(L.load().f3r_attention(_ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, _ptr(lse), batch, heads, sq, skv,
-                                           float(scale), st.cuda_stream), "f3r_attention")
+        _call("f3r_attention", q, _ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, _ptr(lse), batch, heads, sq, skv,
+              float(scale))
     if timer is not None:
         e1.record(st)
         timer.append((batch, heads, sq, skv, e0, e1))
@@ -222,12 +213,10 @@ def attention_x3(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch:
     _chk(q, F32, "q"); _chk(kv, F32, "kv"); _chk(out, F32, "out")
     ldq, ldkv, ldo = q.shape[-1], kv.shape[-1], out.shape[-1]
     assert q.numel() == batch * sq * ldq and kv.numel() == batch * skv * ldkv and out.numel() == batch * sq * ldo
-    lib = L.load()
-    nbytes = int(lib.f3r_attention_x3_workspace(batch, heads, sq, skv))
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)  # caching allocator: >= 512-byte aligned
-    with _on_device(q):
-        L.check(lib.f3r_attention_x3(_ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, _ptr(lse), _ptr(ws), nbytes, batch,
-                                     heads, sq, skv, float(scale), _stream(q)), "f3r_attention_x3")
+    nbytes = L.load().f3r_attention_x3_workspace(batch, heads, sq, skv)
+    ws = _scratch(nbytes, q.device)
+    _call("f3r_attention_x3", q, _ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, _ptr(lse), _ptr(ws), nbytes, batch, heads,
+          sq, skv, float(scale))
 
 
 def transformer_blocks(x: torch.Tensor, blocks, *, batch: int, seq: int, heads: int, eps: float, scale: float,
@@ -244,25 +233,21 @@ def transformer_blocks(x: torch.Tensor, blocks, *, batch: int, seq: int, heads: 
                         ("qkv_w", b.qkv_w), ("qkv_b", b.qkv_b), ("proj_w", b.proj_w), ("proj_b", b.proj_b),
                         ("fc1_w", b.fc1_w), ("fc1_b", b.fc1_b), ("fc2_w", b.fc2_w), ("fc2_b", b.fc2_b)):
             setattr(arr[i], name, _ptr(t))
-    lib = L.load()
     rows = batch * seq
     assert x.numel() == rows * D
-    nbytes = int(lib.f3r_transformer_workspace(rows, D, hidden))
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-    with _on_device(x):
-        L.check(lib.f3r_transformer_blocks(arr, len(blocks), _ptr(x), batch, seq, D, heads, hidden, float(eps), float(scale),
-                                           rope["gw"] if rope else 0, rope["P"] if rope else 0,
-                                           _ptr(rope["cos"]) if rope else None, _ptr(rope["sin"]) if rope else None,
-                                           _ptr(ws), nbytes, _stream(x)), "f3r_transformer_blocks")
+    nbytes = L.load().f3r_transformer_workspace(rows, D, hidden)
+    ws = _scratch(nbytes, x.device)
+    _call("f3r_transformer_blocks", x, arr, len(blocks), _ptr(x), batch, seq, D, heads, hidden, float(eps), float(scale),
+          rope["gw"] if rope else 0, rope["P"] if rope else 0, _ptr(rope["cos"]) if rope else None,
+          _ptr(rope["sin"]) if rope else None, _ptr(ws), nbytes)
 
 
 def layernorm(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float, out: torch.Tensor):
     _chk(x, F32, "x"); _chk(w, F32, "w"); _chk(b, F32, "b")
     assert out.dtype in (BF16, F32) and out.is_contiguous() and out.numel() == x.numel()
     dim = x.shape[-1]
-    with _on_device(x):
-        L.check(L.load().f3r_layernorm(_ptr(x), _ptr(w), _ptr(b), _ptr(out), int(out.dtype == F32), x.numel() // dim,
-                                       dim, float(eps), _stream(x)), "f3r_layernorm")
+    _call("f3r_layernorm", x, _ptr(x), _ptr(w), _ptr(b), _ptr(out), int(out.dtype == F32), x.numel() // dim, dim,
+          float(eps))
 
 
 def im2col_patch(img: torch.Tensor, out: torch.Tensor):
@@ -270,31 +255,25 @@ def im2col_patch(img: torch.Tensor, out: torch.Tensor):
     assert out.dtype in (BF16, F32) and out.is_contiguous()
     n, c, h, w = img.shape
     assert c == 3 and out.numel() == n * (h // 16) * (w // 16) * 768
-    with _on_device(img):
-        L.check(L.load().f3r_im2col_patch(_ptr(img), _ptr(out), int(out.dtype == F32), n, h, w, _stream(img)),
-                "f3r_im2col_patch")
+    _call("f3r_im2col_patch", img, _ptr(img), _ptr(out), int(out.dtype == F32), n, h, w)
 
 
 def im2col3x3s2(x: torch.Tensor, out: torch.Tensor, n: int, h: int, w: int, c: int, ho: int, wo: int):
     _chk(x, BF16, "x"); _chk(out, BF16, "out")
     assert x.numel() == n * h * w * c and out.numel() == n * ho * wo * 9 * c
-    with _on_device(x):
-        L.check(L.load().f3r_im2col3x3s2(_ptr(x), _ptr(out), n, h, w, c, ho, wo, _stream(x)), "f3r_im2col3x3s2")
+    _call("f3r_im2col3x3s2", x, _ptr(x), _ptr(out), n, h, w, c, ho, wo)
 
 
 def upsample2x(x: torch.Tensor, out: torch.Tensor, n: int, h: int, w: int, c: int, ho: int, wo: int):
     assert x.dtype in (BF16, F32) and x.dtype == out.dtype and x.is_contiguous() and out.is_contiguous()
     assert x.numel() == n * h * w * c and out.numel() == n * ho * wo * c
-    with _on_device(x):
-        L.check(L.load().f3r_upsample2x(_ptr(x), _ptr(out), int(x.dtype == F32), n, h, w, c, ho, wo, _stream(x)),
-                "f3r_upsample2x")
+    _call("f3r_upsample2x", x, _ptr(x), _ptr(out), int(x.dtype == F32), n, h, w, c, ho, wo)
 
 
 def cast_bf16(x: torch.Tensor, out: torch.Tensor):
     _chk(x, F32, "x"); _chk(out, BF16, "out")
     assert x.numel() == out.numel()
-    with _on_device(x):
-        L.check(L.load().f3r_cast_bf16(_ptr(x), _ptr(out), x.numel(), _stream(x)), "f3r_cast_bf16")
+    _call("f3r_cast_bf16", x, _ptr(x), _ptr(out), x.numel())
 
 
 # ------------------------------------------------------------------ geometry tail (csrc/geometry.cu)
@@ -303,9 +282,7 @@ def conf_quantile(conf: torch.Tensor, q: float) -> torch.Tensor:
     _chk(conf, F32, "conf")
     assert conf.dim() == 2
     thr = torch.empty(conf.shape[0], dtype=F32, device=conf.device)
-    with _on_device(conf):
-        L.check(L.load().f3r_conf_quantile(_ptr(conf), conf.shape[0], conf.shape[1], float(q), _ptr(thr), _stream(conf)),
-                "f3r_conf_quantile")
+    _call("f3r_conf_quantile", conf, _ptr(conf), conf.shape[0], conf.shape[1], float(q), _ptr(thr))
     return thr
 
 
@@ -322,13 +299,11 @@ def similarity_fit(x: torch.Tensor, y: torch.Tensor, conf: Optional[torch.Tensor
     if valid is not None:
         _chk(valid, torch.uint8, "valid")
         assert valid.shape == (views, n)
-    lib = L.load()
-    nbytes = lib.f3r_similarity_fit_workspace(views)
-    ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=x.device)
+    nbytes = L.load().f3r_similarity_fit_workspace(views)
+    ws = _scratch(nbytes, x.device)
     rts = torch.empty(views, 13, dtype=F32, device=x.device)
-    with _on_device(x):
-        L.check(lib.f3r_similarity_fit(_ptr(x), _ptr(y), _ptr(conf), _ptr(thr), _ptr(valid), views, n, _ptr(rts), _ptr(ws),
-                                       nbytes, _stream(x)), "f3r_similarity_fit")
+    _call("f3r_similarity_fit", x, _ptr(x), _ptr(y), _ptr(conf), _ptr(thr), _ptr(valid), views, n, _ptr(rts), _ptr(ws),
+          nbytes)
     return rts
 
 
@@ -341,8 +316,7 @@ def similarity_apply(x: torch.Tensor, rts: torch.Tensor, out: Optional[torch.Ten
         out = torch.empty_like(x)
     _chk(out, F32, "out")
     assert out.shape == x.shape
-    with _on_device(x):
-        L.check(L.load().f3r_similarity_apply(_ptr(x), _ptr(rts), _ptr(out), views, n, _stream(x)), "f3r_similarity_apply")
+    _call("f3r_similarity_apply", x, _ptr(x), _ptr(rts), _ptr(out), views, n)
     return out
 
 
@@ -359,11 +333,9 @@ def focal_weiszfeld(pts: torch.Tensor, conf: Optional[torch.Tensor] = None, thr:
     if pp is not None:
         _chk(pp, F32, "pp")
         assert pp.shape == (views, 2)
-    lib = L.load()
-    nbytes = lib.f3r_focal_workspace(views)
-    ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=pts.device)
+    nbytes = L.load().f3r_focal_workspace(views)
+    ws = _scratch(nbytes, pts.device)
     focal = torch.empty(views, dtype=F32, device=pts.device)
-    with _on_device(pts):
-        L.check(lib.f3r_focal_weiszfeld(_ptr(pts), _ptr(conf), _ptr(thr), _ptr(pp), views, h, w, int(iters), _ptr(focal),
-                                        _ptr(ws), nbytes, _stream(pts)), "f3r_focal_weiszfeld")
+    _call("f3r_focal_weiszfeld", pts, _ptr(pts), _ptr(conf), _ptr(thr), _ptr(pp), views, h, w, int(iters), _ptr(focal),
+          _ptr(ws), nbytes)
     return focal

@@ -76,10 +76,9 @@ size_t f3r_gemm_desc_size(void);
 /* Number of kernels launched through this library by the calling process so far. */
 uint64_t f3r_launch_count(void);
 
-/* Tuning knobs for A/B measurements (process-wide).  "attn_emu" = how many of every 8 exponential pairs of the
- * attention softmax are evaluated on the FMA pipe instead of MUFU.EX2 (0..3, -1 = built-in default); "attn_split" =
- * softmax threads per query row (1 or 2, -1 = default); "pdl" = 1 / 0: launch the GEMM / attention / LayerNorm chain with
- * programmatic dependent launch (successor prologues overlap predecessor tails; default 1, env F3R_PDL=0 disables). */
+/* Tuning knobs for A/B measurements (process-wide).  The only option is "pdl" = 1 / 0: launch the GEMM / attention /
+ * LayerNorm chain with programmatic dependent launch (successor prologues overlap predecessor tails; default 1, env
+ * F3R_PDL=0 disables).  Any other name is an error. */
 int f3r_set_option(const char* name, int32_t value);
 
 int f3r_gemm(const f3r_gemm_desc* d, void* stream);
@@ -90,11 +89,12 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream);
 int f3r_attention(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo, float* lse,
                   int32_t batch, int32_t heads, int32_t sq, int32_t skv, float scale, void* stream);
 
-/* Key-slice form of f3r_attention, for (a) filling the SMs when batch*heads*ceil(sq/128) is small and (b) attending
+/* Key-slice form of f3r_attention, for (a) filling the SMs when batch*heads*ceil(sq/192) is small and (b) attending
  * to key ranges as they arrive over NVLink (sequence-parallel decoder, fast3r_b200/parallel.py): attends the queries to
  * the keys [kv_row0, kv_row0 + skv) of a kv buffer of kv_rows_total rows per batch, cut into n_split slices (one CTA each
- * per 256-row query tile); slice s writes its softmax-normalised fp32 output into part_o[part_base + s] (layout
- * [slot, batch*sq, heads*64]) and its log-sum-exp into part_lse[part_base + s] ([slot, batch, heads, sq]).
+ * per query tile of ATT_Q_TILE = 192 rows, csrc/f3r_kernels.h); slice s writes its softmax-normalised fp32 output into
+ * part_o[part_base + s] (layout [slot, batch*sq, heads*64]) and its log-sum-exp into part_lse[part_base + s]
+ * ([slot, batch, heads, sq]).
  * f3r_attention_merge combines n_parts slots into the exact softmax over the union of their keys (bf16 out). */
 int f3r_attention_partial(const void* q, int32_t ldq, const void* kv, int32_t ldkv, int32_t kv_rows_total,
                           int32_t kv_row0, int32_t skv, int32_t n_split, float* part_o, float* part_lse,
