@@ -399,6 +399,25 @@ int f3r_ingest_rgb8(const uint8_t* src, int32_t h, int32_t w, int32_t oh, int32_
                                   static_cast<cudaStream_t>(stream)), "f3r_ingest_rgb8");
 }
 
+int f3r_jpeg_probe(const uint8_t* data, size_t size, f3r_jpeg_info* info) {
+  if (!info || (!data && size)) return fail("f3r_jpeg_probe: null operand");
+  const char* why = f3r::jpeg_probe(data, size, info);
+  if (info->status != F3R_JPEG_SUPPORTED) fail("f3r_jpeg_probe: %s", why ? why : "");
+  return 0;
+}
+
+int f3r_jpeg_decode(const uint8_t* data, size_t size, const uint8_t* data_dev, int32_t orientation, int32_t rotate_cw90,
+                    int32_t left, int32_t top, int32_t out_w, int32_t out_h, uint8_t* out, int32_t* status_dev,
+                    void* workspace, size_t workspace_bytes, void* stream) {
+  if (!data || !data_dev || !out || !status_dev || !workspace) return fail("f3r_jpeg_decode: null operand");
+  int launches = 0;
+  const char* err = f3r::launch_jpeg_decode(data, size, data_dev, orientation, rotate_cw90, left, top, out_w, out_h, out,
+                                            status_dev, workspace, workspace_bytes, static_cast<cudaStream_t>(stream),
+                                            &launches);
+  g_launches += launches;
+  return err ? fail("f3r_jpeg_decode: %s", err) : 0;
+}
+
 // ---------------------------------------------------------------- geometry tail
 int f3r_conf_quantile(const float* conf, int32_t views, int32_t n, float q, float* thr, void* stream) {
   if (!conf || !thr) return fail("f3r_conf_quantile: null operand");

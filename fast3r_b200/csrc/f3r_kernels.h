@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/fast3r_b200.h"
+
 namespace f3r {
 
 // 1: launch the hot-chain kernels with programmatic stream serialization (PDL); F3R_PDL=0 / f3r_set_option("pdl", 0) disable
@@ -88,6 +90,12 @@ cudaError_t launch_im2col3x3s2(const void* in, void* out, int n, int H, int W, i
 cudaError_t launch_upsample2x(const void* in, void* out, int f32, int n, int H, int W, int C, int Ho, int Wo,
                               int Hfull, int Wfull, cudaStream_t stream);
 cudaError_t launch_cast_bf16(const float* in, void* out, size_t n, cudaStream_t stream);
+
+// baseline JPEG decode (jpeg.cu); both return nullptr or the reason of the failure
+const char* jpeg_probe(const uint8_t* data, size_t size, f3r_jpeg_info* info);
+const char* launch_jpeg_decode(const uint8_t* data, size_t size, const uint8_t* data_dev, int orientation, int rotate_cw90,
+                               int left, int top, int out_w, int out_h, uint8_t* out, int32_t* status, void* workspace,
+                               size_t workspace_bytes, cudaStream_t stream, int* launches);
 
 // image ingest (ingest.cu)
 int resample_ksize(int in_size, int out_size, int filter);

@@ -42,6 +42,15 @@ class BlockWeights(C.Structure):
                                           "fc1_w", "fc1_b", "fc2_w", "fc2_b")]
 
 
+JPEG_SUPPORTED, JPEG_UNSUPPORTED, JPEG_MALFORMED = range(3)
+
+
+class JpegInfo(C.Structure):
+    _fields_ = [("status", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("components", C.c_int32),
+                ("h_samp", C.c_int32), ("v_samp", C.c_int32), ("restart_interval", C.c_int32), ("segments", C.c_int32),
+                ("scan_offset", C.c_size_t), ("scan_bytes", C.c_size_t), ("workspace_bytes", C.c_size_t)]
+
+
 # name -> (restype, argtypes), one entry per prototype of include/fast3r_b200.h, in header order.  ctypes does not check
 # these against the C side: tests/test_cabi_bindings_cpu.py compares every entry with the header.  Device pointers and
 # the cudaStream_t are void*.
@@ -69,6 +78,8 @@ _API = {
     "f3r_resample_coeffs": (C.c_int, [_I32, _I32, _I32, _P, _P]),
     "f3r_ingest_rgb8": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _I32, _I32, _P, _P, _I32, _P, _I32, _I32, _I32,
                                   _I32, _P, _P]),
+    "f3r_jpeg_probe": (C.c_int, [_P, _SIZE, C.POINTER(JpegInfo)]),
+    "f3r_jpeg_decode": (C.c_int, [_P, _SIZE, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _SIZE, _P]),
     "f3r_conf_quantile": (C.c_int, [_P, _I32, _I32, _F32, _P, _P]),
     "f3r_similarity_fit_workspace": (_SIZE, [_I32]),
     "f3r_similarity_fit": (C.c_int, [_P, _P, _P, _P, _P, _I32, _I32, _P, _P, _SIZE, _P]),

@@ -151,6 +151,35 @@ int f3r_ingest_rgb8(const uint8_t* src, int32_t h, int32_t w, int32_t oh, int32_
                     int32_t hks, int32_t h_span_max, const int32_t* vb, const int32_t* vk, int32_t vks, uint8_t* tmp,
                     int32_t left, int32_t top, int32_t cw, int32_t ch, float* out, void* stream);
 
+/* ---- baseline JPEG decode, bit-exact with Pillow's (libjpeg-turbo: accurate integer IDCT, fancy upsampling, JCS_RGB
+ * output).  The GPU decodes Huffman-coded 8-bit sequential JPEGs (SOF0, SOF1) with one component or three YCbCr
+ * components at 4:4:4, 4:2:2 or 4:2:0, with or without restart markers; the caller keeps every other file on its host
+ * decoder.
+ * f3r_jpeg_probe (HOST function, no CUDA call) parses the `size` bytes at `data` and fills *info: status
+ * F3R_JPEG_SUPPORTED, F3R_JPEG_UNSUPPORTED or F3R_JPEG_MALFORMED (the reason in f3r_last_error()), the image size and,
+ * when supported, the scan layout and the device workspace f3r_jpeg_decode needs.  Returns non-zero only for bad
+ * arguments.
+ * f3r_jpeg_decode parses the same host bytes again (header only) and decodes the DEVICE copy data_dev of those bytes into
+ * out, uint8 [out_h][out_w][3] RGB: the decoded image after ImageOps.exif_transpose for `orientation` (1..8; anything
+ * else is 1), then rotate(-90, expand=True) when rotate_cw90 != 0, then the crop box (left, top, out_w, out_h).
+ * workspace: info.workspace_bytes, 256-byte aligned.  The stream is decoded asynchronously: *status_dev (a device
+ * int32) becomes 0, or a combination of the F3R_JPEG_ERR_* bits when the entropy-coded data is inconsistent (the image in
+ * out is then undefined; the file should be decoded on the host instead). */
+enum { F3R_JPEG_SUPPORTED = 0, F3R_JPEG_UNSUPPORTED = 1, F3R_JPEG_MALFORMED = 2 };
+enum { F3R_JPEG_ERR_SYNC = 1, F3R_JPEG_ERR_CODE = 2, F3R_JPEG_ERR_COUNT = 4, F3R_JPEG_ERR_TRUNC = 8 };
+typedef struct f3r_jpeg_info {
+  int32_t status;
+  int32_t width, height, components;
+  int32_t h_samp, v_samp;            /* luma sampling factors (chroma is 1x1)                                        */
+  int32_t restart_interval, segments; /* MCUs per restart interval (0: none), entropy-coded segments                  */
+  size_t scan_offset, scan_bytes;    /* the entropy-coded data: bytes [scan_offset, scan_offset + scan_bytes)        */
+  size_t workspace_bytes;
+} f3r_jpeg_info;
+int f3r_jpeg_probe(const uint8_t* data, size_t size, f3r_jpeg_info* info);
+int f3r_jpeg_decode(const uint8_t* data, size_t size, const uint8_t* data_dev, int32_t orientation, int32_t rotate_cw90,
+                    int32_t left, int32_t top, int32_t out_w, int32_t out_h, uint8_t* out, int32_t* status_dev,
+                    void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- geometry tail (SURVEY §8 f2, first slice): what every caller runs on the forward's outputs before poses.
  * A "view" below is one (view, batch item) pointmap of n = H*W pixels; all arrays are DEVICE pointers, fp32, view-major.
  *
