@@ -228,7 +228,10 @@ static int attention_impl(const char* what, const void* q, int32_t ldq, const vo
     if (make_tmap(&tq, q, 3, dims, str, box)) return 1;
   }
   {
-    const uint64_t dims[3] = {static_cast<uint64_t>(heads) * 128, static_cast<uint64_t>(kv_rows_total),
+    // the map ends where the key range ends (the batch stride stays kv_rows_total rows): the last key block of the range
+    // is a full 128-row load, and the rows past the range come back zero-filled, never as whatever follows in the
+    // buffer.  Their scores are masked, but their V rows enter the PV product with P = 0, and 0 * NaN would be NaN.
+    const uint64_t dims[3] = {static_cast<uint64_t>(heads) * 128, static_cast<uint64_t>(kv_row0 + skv),
                               static_cast<uint64_t>(batch)};
     const uint64_t str[2] = {static_cast<uint64_t>(ldkv) * 2, static_cast<uint64_t>(ldkv) * 2 * kv_rows_total};
     const uint32_t box[3] = {64, 128, 1};

@@ -734,16 +734,19 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         for i, im in enumerate(imgs):
             groups.setdefault(tuple(im.shape[-2:]), []).append(i)
         sp = self.sp_group
-        if sp is not None and len(groups) > 1:
-            raise NotImplementedError("fast3r_b200: sequence parallel needs views of one resolution")
         device = views[0]["img"].device
         if sp is not None and device.type != "cuda":
             device = next(self.parameters()).device  # sharded forward: host views are uploaded per rank below
         P_ = self._pack(device)
-        lo, hi = (0, N) if sp is None else sp.view_range(N)
+        tokens = [(im.shape[-2] // ps) * (im.shape[-1] // ps) for im in imgs]
+        off = list(accumulate(tokens, initial=0))  # first token of each view in a sample's sequence
+        # sequence parallel: contiguous views per rank, balanced by token count (views of different resolutions)
+        lo, hi = (0, N) if sp is None else sp.view_range(N, tokens)
         enc = []  # per group: ((H, W), this rank's views, their encoder tokens in (view, b, patch) order, P, gh, gw)
         for shape, idxs in groups.items():
             idxs = [i for i in idxs if lo <= i < hi]
+            if not idxs:  # no view of this resolution on this rank
+                continue
             x = torch.cat([imgs[i].to(device, non_blocking=True) for i in idxs], dim=0).to(dtype=F32).contiguous()
             enc.append((shape, idxs) + self._encode(x, P_))
         if profiling:
@@ -762,7 +765,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         t2 = time.time()
         # decoder input: the tokens of each sample in (view, patch) order; to_heads[g] takes a decoder output back to
         # group g's (view, b, patch) order, the order of the head input (fast3r.py:385-398)
-        if len(enc) == 1:  # one image id per view
+        if len(groups) == 1:  # one image id per view
             (_, idxs, feats, P, _, _), = enc
             seq, tok_per_img, ids = len(idxs) * P, P, ids[:, lo:hi].contiguous()
             if B == 1:
@@ -772,25 +775,24 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
                 swap = lambda t, a, b: t.view(a, b, P, -1).permute(1, 0, 2, 3).contiguous().view(a * b * P, -1)  # noqa: E731
                 feats_bnp, to_heads = swap(feats, n, B), [lambda t: swap(t, B, n)]
         else:  # one image-index row per token; one index_copy / index_select per group instead of per-view slices
-            tok = [0] * N
-            for _, idxs, _, P, _, _ in enc:
-                for i in idxs:
-                    tok[i] = P
-            off = list(accumulate(tok, initial=0))
-            seq, tok_per_img = off[-1], 0
+            t0 = off[lo]  # this rank's tokens are [off[lo], off[hi]) of each sample's sequence
+            seq, tok_per_img = off[hi] - t0, 0
             feats_bnp = torch.empty(B * seq, self.encoder.embed_dim, dtype=P_.adt, device=device)
             tok_ids = torch.empty(B, seq, dtype=torch.int32)
             to_heads = []
             for _, idxs, feats, P, _, _ in enc:
-                base = torch.tensor([off[i] for i in idxs], dtype=torch.long)  # (n_g,)
+                base = torch.tensor([off[i] - t0 for i in idxs], dtype=torch.long)  # (n_g,)
                 r = (base[:, None, None] + torch.arange(B, dtype=torch.long)[None, :, None] * seq
                      + torch.arange(P, dtype=torch.long)[None, None, :]).reshape(-1).to(device)  # (n_g, B, P) order
                 feats_bnp.index_copy_(0, r, feats)
                 for i in idxs:
-                    tok_ids[:, off[i]: off[i] + P] = ids[:, i:i + 1].to(torch.int32)
+                    tok_ids[:, off[i] - t0: off[i] - t0 + P] = ids[:, i:i + 1].to(torch.int32)
                 to_heads.append(lambda t, r=r: t.index_select(0, r))
             ids = tok_ids.reshape(-1)
-        kvx = sp.make_kv_exchange(B, seq, self.decoder.embed_dim) if sp is not None else None
+        kvx = None
+        if sp is not None:
+            kvx = sp.make_kv_exchange(B, seq, self.decoder.embed_dim, rows=[off[b] - off[a] for a, b in sp.ranges],
+                                      mixed=len(groups) > 1)
         dec_out = self._decode(feats_bnp, ids, B, seq, tok_per_img, P_, kv_exchange=kvx)
         if profiling:
             _sync(device)
@@ -810,7 +812,8 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
                 for k in list(r):
                     r[k] = r[k].swapaxes(1, 2)
         if sp is not None and sp.gather_preds:
-            final_results = sp.gather_results(final_results, N, B, H, W, device)
+            final_results = sp.gather_results(final_results, N, B, H, W, device,
+                                              shapes=[v["img"].shape[-2:] for v in views])
         if profiling:
             _sync(device)
             t_end = time.time()

@@ -2,15 +2,17 @@
 
 The reference has no counterpart (SURVEY.md §2a: no TP/PP/SP anywhere); the single-device result is the oracle.
 Partitioning (SURVEY.md §8(e)): rank r owns a contiguous range of views, i.e. a contiguous token range of the
-N*P-token sequence.  Encoder blocks, LayerNorm, all linears and the DPT heads are token/view-local and need no
-communication; only the global attention couples ranks: each decoder layer all-gathers K|V (bf16, S_local x 2D)
+sequence; with views of different resolutions the ranges balance the token counts (shard_views_weighted).  Encoder
+blocks, LayerNorm, all linears and the DPT heads are token/view-local and need no communication; only the global attention couples ranks: each decoder layer all-gathers K|V (bf16, S_local x 2D)
 over NCCL/NVLink and every rank attends its local queries against all keys.  The image-index ids drawn by rank 0 are
 broadcast to all ranks so the result equals the single-device forward whatever the per-rank RNG states are.
 """
 from __future__ import annotations
 
+import math
 import os
-from typing import List, Tuple
+from itertools import accumulate
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 import torch.distributed as dist
@@ -41,6 +43,65 @@ def shard_views(num_views: int, world: int) -> List[Tuple[int, int]]:
     return out
 
 
+def shard_views_weighted(tokens: Sequence[int], world: int) -> List[Tuple[int, int]]:
+    """Contiguous view ranges, at least one view per rank, that minimise the largest per-rank token count (the linear
+    partition problem, solved exactly).  `tokens`: tokens per view.  Among the optimal partitions each rank takes the
+    fewest views that reach an equal share of the tokens still unassigned, so equal token counts give exactly
+    shard_views(len(tokens), world)."""
+    n = len(tokens)
+    if n < world:
+        raise ValueError(f"sequence parallel needs at least one view per rank ({n} views, {world} ranks)")
+    pre = list(accumulate(tokens, initial=0))
+
+    def parts_needed(cap: int) -> List[int]:
+        """need[i]: fewest ranges of at most `cap` tokens that cover views [i, n) (greedy from i is optimal)."""
+        need, j = [0] * (n + 1), n
+        for i in range(n - 1, -1, -1):
+            while pre[j] - pre[i] > cap:
+                j -= 1
+            need[i] = 1 + need[j]
+        return need
+
+    lo_cap, hi_cap = max(tokens), pre[n]   # the optimal largest load lies in [lo_cap, hi_cap]
+    while lo_cap < hi_cap:
+        mid = (lo_cap + hi_cap) // 2
+        if parts_needed(mid)[0] <= world:
+            hi_cap = mid
+        else:
+            lo_cap = mid + 1
+    cap, need = lo_cap, parts_needed(lo_cap)
+    out, a = [], 0
+    for r in range(world):
+        left = world - r - 1   # ranks after this one
+        if left == 0:
+            out.append((a, n))
+            break
+        # feasible ends e: this range fits the cap, and [e, n) still splits into `left` non-empty ranges within the cap
+        ends = [e for e in range(a + 1, n - left + 1) if pre[e] - pre[a] <= cap and need[e] <= left]
+        share = (pre[n] - pre[a]) / (left + 1)
+        e = next((e for e in ends if pre[e] - pre[a] >= share), ends[-1])
+        out.append((a, e))
+        a = e
+    return out
+
+
+def peer_key_ranges(rows: List[int], rank: int) -> List[Tuple[int, int]]:
+    """Key ranges (first row, rows) that `rank` attends in the overlapped K|V exchange, in a gather buffer that holds each
+    rank's rows in a slot of max(rows) rows: its own rows first, then the other ranks' rows in rank order, never a
+    padding row.  Other ranks' slots that follow each other with no padding in between form one range (so with equal
+    rows: the ranks before and the ranks after this one)."""
+    mx = max(rows)
+    peers: List[Tuple[int, int]] = []
+    for p, n in enumerate(rows):
+        if p == rank:
+            continue
+        if peers and p - 1 != rank and peers[-1][0] + peers[-1][1] == p * mx:
+            peers[-1] = (peers[-1][0], peers[-1][1] + n)
+        else:
+            peers.append((p * mx, n))
+    return [(rank * mx, rows[rank])] + peers
+
+
 def assemble_kv(gathered: torch.Tensor, batch: int, rows: List[int]) -> torch.Tensor:
     """gathered: (world, batch * max_rows, C) padded per-rank K|V blocks, each laid out (b, s_local).
     Returns (batch * sum(rows), C) laid out (b, s_global) with ranks concatenated in order."""
@@ -56,23 +117,28 @@ def assemble_kv(gathered: torch.Tensor, batch: int, rows: List[int]) -> torch.Te
 class KVExchange:
     """K|V exchange + global attention of one sequence-parallel decoder forward.
 
-    Fast path (bf16 path, batch 1, equal shards): the QKV GEMM writes this rank's K|V straight into its slot of the
-    gather buffer (`kv_workspace()`); `attend()` starts the NCCL all-gather on a side stream and meanwhile attends the
-    local queries to the LOCAL keys; when the gather has landed it attends to the key ranges of the other ranks and merges
-    the partial results by their log-sum-exp (exact softmax over the union, f3r_attention_merge).  The exchange is hidden
+    Fast path (bf16 path, batch 1, equal shards or views of mixed resolution): the QKV GEMM writes this rank's K|V
+    straight into its slot of the gather buffer (`kv_workspace()`); every slot has the rows of the largest rank, so ranks
+    with fewer tokens leave padding at its end.  `attend()` starts the NCCL all-gather on a side stream and meanwhile
+    attends the local queries to the LOCAL keys; when the gather has landed it attends to the real rows of the other ranks
+    (peer_key_ranges) and merges the partial results by their log-sum-exp (exact softmax over the union,
+    f3r_attention_merge).  The exchange is hidden
     behind the local-chunk attention and every launch is key-sliced to fill the 132 SMs (ops.pick_kv_split).
-    General path (batch > 1, uneven shards, parity precision, CPU emulator): all-gather, then one attention call."""
+    General path (batch > 1, parity precision, CPU emulator, views of one resolution in uneven shards): all-gather, then
+    one attention call, bit-identical to the single-device forward.  `mixed`: the views have different resolutions, so the
+    rows are almost never equal and the overlapped path takes uneven rows."""
 
-    def __init__(self, sp, batch: int, s_local: int, dim: int, rows: List[int]):
+    def __init__(self, sp, batch: int, s_local: int, dim: int, rows: List[int], mixed: bool = False):
         self.sp, self.batch, self.s_local, self.dim, self.rows = sp, batch, s_local, dim, rows
         self.mx, self.s_total = max(rows), sum(rows)
         self.even = all(r == self.mx for r in rows)
+        self.mixed = mixed
         self.buf = None
         self.pad = None
         self.comm_stream = None
         self.parts = None
         self.layer = 0
-        self.sym = None          # symmetric-memory transport: (2, s_local, C) K|V slots of this rank, double-buffered per layer
+        self.sym = None          # symmetric-memory transport: (2, mx, C) K|V slots of this rank, double-buffered per layer
         self.sym_state = None    # None: not tried yet, True / False
 
     def _setup_symmetric(self, like: torch.Tensor) -> bool:
@@ -93,9 +159,9 @@ class KVExchange:
             import torch.distributed._symmetric_memory as symm
             group = sp.group if sp.group is not None else dist.group.WORLD
             C = 2 * self.dim
-            sym = symm.empty((2, self.s_local, C), dtype=like.dtype, device=like.device)
+            sym = symm.empty((2, self.mx, C), dtype=like.dtype, device=like.device)
             hdl = symm.rendezvous(sym, group)
-            peers = [hdl.get_buffer(r, (2, self.s_local, C), like.dtype) for r in range(sp.world)]
+            peers = [hdl.get_buffer(r, (2, self.mx, C), like.dtype) for r in range(sp.world)]
             streams = [torch.cuda.Stream(device=like.device) for _ in range(max(1, min(4, sp.world - 1)))]
         except Exception as e:  # noqa: BLE001
             ok = 0
@@ -119,7 +185,8 @@ class KVExchange:
                 self.comm_stream = torch.cuda.Stream(device=like.device)
 
     def fast(self, dtype, device) -> bool:
-        return self.even and self.batch == 1 and dtype == torch.bfloat16 and device.type == "cuda" and self.sp.overlap
+        return ((self.even or self.mixed) and self.batch == 1 and dtype == torch.bfloat16 and device.type == "cuda"
+                and self.sp.overlap)
 
     def kv_workspace(self, dtype, device):
         """Where the QKV GEMM of the NEXT decoder layer should write this rank's K|V (None: any buffer; attend() copies).
@@ -154,7 +221,7 @@ class KVExchange:
         self.layer += 1
         slot = self.sym[par] if use_sym else self.buf[sp.rank]
         if kv.data_ptr() != slot.data_ptr():
-            slot.copy_(kv)
+            slot[:self.s_local].copy_(kv)
         compute = torch.cuda.current_stream(kv.device)
         tm = sp.timers  # optional CUDA-event trace of the phases (bench.py): list of per-call event tuples
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(6)] if tm is not None else None
@@ -176,11 +243,14 @@ class KVExchange:
                 st = self.copy_streams[(i - 1) % len(self.copy_streams)]
                 st.wait_event(ready)
                 with torch.cuda.stream(st):
-                    self.buf[p_].copy_(self.peers[p_][par], non_blocking=True)
+                    n = self.rows[p_]
+                    self.buf[p_][:n].copy_(self.peers[p_][par][:n], non_blocking=True)
             for st in self.copy_streams:
                 self.comm_stream.wait_stream(st)
             if ev:
                 ev[5].record(self.comm_stream)
+            # the real rows of every rank (the whole buffer when the rows are equal); padding is not pulled
+            sp.bytes_exchanged += self.s_total * C * self.buf.element_size()
         else:
             with torch.cuda.stream(self.comm_stream):
                 if ev:
@@ -188,40 +258,53 @@ class KVExchange:
                 _all_gather_into(self.buf.view(-1, C), slot, group=sp.group)
                 if ev:
                     ev[5].record(self.comm_stream)
-        sp.bytes_exchanged += self.buf.numel() * self.buf.element_size()
-        S, sl = self.s_total, self.s_local
-        lo, hi = sp.rank * sl, (sp.rank + 1) * sl
-        units = attention_units(1, heads, sl)
-        # local keys first (straight from this rank's slot), then the other ranks' ranges of the gather buffer
-        ranges = [(lo, sl)] + [r for r in ((0, lo), (hi, S - hi)) if r[1] > 0]
-        splits = [ops.pick_kv_split(units, (n + 127) // 128) for _, n in ranges]
-        slots = sum(splits)
-        if self.parts is None or self.parts[0].shape[0] < slots:
-            self.parts = (torch.empty(slots, sl, heads * 64, dtype=torch.float32, device=kv.device),
-                          torch.empty(slots, 1, heads, sl, dtype=torch.float32, device=kv.device))
-        part_o, part_lse = self.parts
-        kv_all = self.buf.view(-1, C)
-        base = 0
-        for i, ((row0, n), ns) in enumerate(zip(ranges, splits)):
-            if i == 1:
-                if ev:
-                    ev[1].record(compute)
-                compute.wait_stream(self.comm_stream)  # the other ranks' keys have landed
-            if i == 0 and use_sym:   # the local keys are read where the QKV GEMM wrote them
-                ops.attention_partial(q, slot, part_o, part_lse, part_base=base, n_split=ns, batch=1, heads=heads, sq=sl,
-                                      kv_rows_total=sl, kv_row0=0, skv=n, scale=scale)
-            else:
-                ops.attention_partial(q, kv_all, part_o, part_lse, part_base=base, n_split=ns, batch=1, heads=heads,
-                                      sq=sl, kv_rows_total=S, kv_row0=row0, skv=n, scale=scale)
-            base += ns
-        if len(ranges) == 1:
-            compute.wait_stream(self.comm_stream)
+            sp.bytes_exchanged += self.buf.numel() * self.buf.element_size()   # the all-gather moves the padding too
+
+        def peers_landed():
+            if ev:
+                ev[1].record(compute)
+            compute.wait_stream(self.comm_stream)  # the other ranks' keys have landed
+
+        # with symmetric memory the local keys are read where the QKV GEMM wrote them
+        slots = self.partials(ops, q, slot[:self.s_local] if use_sym else None, heads=heads, scale=scale,
+                              peers_landed=peers_landed)
         if ev:
             ev[2].record(compute)
-        ops.attention_merge(part_o, part_lse, slots, att, batch=1, heads=heads, sq=sl)
+        ops.attention_merge(self.parts[0], self.parts[1], slots, att, batch=1, heads=heads, sq=self.s_local)
         if ev:
             ev[3].record(compute)
             tm.append(ev)
+
+    def partials(self, ops, q, local, *, heads: int, scale: float, peers_landed) -> int:
+        """Overlapped path after the exchange has started: attends the local queries to this rank's keys (`local`, or its
+        slot of the gather buffer when None), calls `peers_landed()`, then attends to the other ranks' real rows of the
+        gather buffer (peer_key_ranges), each range key-sliced (ops.pick_kv_split) into the partial buffers `self.parts`.
+        Returns the number of partials to merge."""
+        sl = self.s_local
+        rows_total = self.sp.world * self.mx
+        units = attention_units(1, heads, sl)
+        ranges = peer_key_ranges(self.rows, self.sp.rank)
+        splits = [ops.pick_kv_split(units, (n + 127) // 128) for _, n in ranges]
+        slots = sum(splits)
+        if self.parts is None or self.parts[0].shape[0] < slots:
+            self.parts = (torch.empty(slots, sl, heads * 64, dtype=torch.float32, device=q.device),
+                          torch.empty(slots, 1, heads, sl, dtype=torch.float32, device=q.device))
+        part_o, part_lse = self.parts
+        kv_all = self.buf.view(-1, self.buf.shape[-1])
+        base = 0
+        for i, ((row0, n), ns) in enumerate(zip(ranges, splits)):
+            if i == 1:
+                peers_landed()
+            if i == 0 and local is not None:
+                ops.attention_partial(q, local, part_o, part_lse, part_base=base, n_split=ns, batch=1, heads=heads, sq=sl,
+                                      kv_rows_total=sl, kv_row0=0, skv=n, scale=scale)
+            else:
+                ops.attention_partial(q, kv_all, part_o, part_lse, part_base=base, n_split=ns, batch=1, heads=heads,
+                                      sq=sl, kv_rows_total=rows_total, kv_row0=row0, skv=n, scale=scale)
+            base += ns
+        if len(ranges) == 1:
+            peers_landed()
+        return slots
 
 
 class SequenceParallel:
@@ -240,11 +323,17 @@ class SequenceParallel:
         self._ranges = None
         self.bytes_exchanged = 0
 
-    def view_range(self, num_views: int) -> Tuple[int, int]:
-        self._ranges = shard_views(num_views, self.world)
-        if any(hi - lo == 0 for lo, hi in self._ranges):
-            raise ValueError(f"sequence parallel needs at least one view per rank ({num_views} views, {self.world} ranks)")
+    def view_range(self, num_views: int, tokens: Optional[Sequence[int]] = None) -> Tuple[int, int]:
+        """This rank's views [lo, hi).  `tokens`: tokens per view (views of different resolutions); the ranges minimise
+        the largest per-rank token count (shard_views_weighted).  Every rank sees the same view shapes, so all ranks
+        agree on the ranges without communicating."""
+        self._ranges = shard_views_weighted(tokens if tokens is not None else [1] * num_views, self.world)
         return self._ranges[self.rank]
+
+    @property
+    def ranges(self) -> List[Tuple[int, int]]:
+        """The view range of every rank, as set by the last view_range call."""
+        return self._ranges
 
     def broadcast_ids(self, ids: torch.Tensor, device) -> torch.Tensor:
         """Every rank uses the image ids drawn by rank 0 of the group (the single-device stream), whatever its own CPU
@@ -257,33 +346,41 @@ class SequenceParallel:
         dist.broadcast(t, src=src, group=self.group)
         return t.cpu()
 
-    def make_kv_exchange(self, batch: int, s_local: int, dim: int):
-        """Per-forward exchange object for the fusion decoder (one per `_decode` call)."""
-        tok_per_view = s_local // (self._ranges[self.rank][1] - self._ranges[self.rank][0])
-        rows = [(hi - lo) * tok_per_view for lo, hi in self._ranges]
-        key = (batch, s_local, dim, tuple(rows))
+    def make_kv_exchange(self, batch: int, s_local: int, dim: int, rows: Optional[List[int]] = None,
+                         mixed: bool = False):
+        """Per-forward exchange object for the fusion decoder (one per `_decode` call).  `rows`: tokens per sample of every
+        rank (default: all views have the token count of this rank's views); `mixed`: views of different resolutions."""
+        if rows is None:
+            tok_per_view = s_local // (self._ranges[self.rank][1] - self._ranges[self.rank][0])
+            rows = [(hi - lo) * tok_per_view for lo, hi in self._ranges]
+        key = (batch, s_local, dim, tuple(rows), mixed)
         if key not in self._kvx:   # buffers (and the symmetric-memory rendezvous) are reused across forwards
-            self._kvx = {key: KVExchange(self, batch, s_local, dim, rows)}
+            self._kvx = {key: KVExchange(self, batch, s_local, dim, list(rows), mixed)}
         self._kvx[key].layer = 0
         return self._kvx[key]
 
-    def gather_results(self, final_results, num_views, batch, H, W, device):
-        """All ranks end up with the preds of every view (API parity with the single-device forward)."""
-        keys = [k for k in ("pts3d_in_other_view", "conf", "pts3d_local", "conf_local")
-                if k in final_results[self._ranges[self.rank][0]]]
-        mxv = max(hi - lo for lo, hi in self._ranges)
+    def gather_results(self, final_results, num_views, batch, H, W, device, shapes=None):
+        """All ranks end up with the preds of every view (API parity with the single-device forward).  `shapes`: the
+        (H, W) of every view's predictions (default: (H, W) for all).  Each rank sends its views' predictions flattened
+        into one buffer padded to the largest rank's and splits what it receives by these shapes, which every rank knows."""
+        shapes = [tuple(s) for s in shapes] if shapes is not None else [(H, W)] * num_views
         lo, hi = self._ranges[self.rank]
+        keys = [k for k in ("pts3d_in_other_view", "conf", "pts3d_local", "conf_local") if k in final_results[lo]]
         out = [dict() for _ in range(num_views)]
         for k in keys:
-            loc = torch.cat([final_results[i][k] for i in range(lo, hi)], dim=0)  # (n_loc*B, ...)
-            tail = loc.shape[1:]
-            send = torch.zeros((mxv * batch,) + tuple(tail), dtype=loc.dtype, device=device)
-            send[: loc.shape[0]] = loc
-            recv = torch.empty((self.world, mxv * batch) + tuple(tail), dtype=loc.dtype, device=device)
-            _all_gather_into(recv.view((-1,) + tuple(tail)), send, group=self.group)
+            chan = tuple(final_results[lo][k].shape[3:])   # (3,) for point maps, () for confidences
+            numel = [batch * h * w * math.prod(chan) for h, w in shapes]
+            sizes = [sum(numel[a:b]) for a, b in self._ranges]
+            loc = torch.cat([final_results[i][k].reshape(-1) for i in range(lo, hi)])
+            send = torch.zeros(max(sizes), dtype=loc.dtype, device=device)
+            send[: loc.numel()] = loc
+            recv = torch.empty(self.world, max(sizes), dtype=loc.dtype, device=device)
+            _all_gather_into(recv.view(-1), send, group=self.group)
             for r, (a, b) in enumerate(self._ranges):
+                o = 0
                 for i in range(a, b):
-                    out[i][k] = recv[r, (i - a) * batch:(i - a + 1) * batch]
+                    out[i][k] = recv[r, o:o + numel[i]].view((batch,) + shapes[i] + chan)
+                    o += numel[i]
         return out
 
 

@@ -91,7 +91,8 @@ int f3r_attention(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void
 
 /* Key-slice form of f3r_attention, for (a) filling the SMs when batch*heads*ceil(sq/192) is small and (b) attending
  * to key ranges as they arrive over NVLink (sequence-parallel decoder, fast3r_b200/parallel.py): attends the queries to
- * the keys [kv_row0, kv_row0 + skv) of a kv buffer of kv_rows_total rows per batch, cut into n_split slices (one CTA each
+ * the keys [kv_row0, kv_row0 + skv) of a kv buffer of kv_rows_total rows per batch (rows outside that range are never
+ * read, so they may hold anything, NaN included), cut into n_split slices (one CTA each
  * per query tile of ATT_Q_TILE = 192 rows, csrc/f3r_kernels.h); slice s writes its softmax-normalised fp32 output into
  * part_o[part_base + s] (layout [slot, batch*sq, heads*64]) and its log-sum-exp into part_lse[part_base + s]
  * ([slot, batch, heads, sq]).
