@@ -467,6 +467,101 @@ int f3r_focal_weiszfeld(const float* pts, const float* conf, const float* thr, c
                                            static_cast<cudaStream_t>(stream)), "f3r_focal_weiszfeld");
 }
 
+// ---------------------------------------------------------------- reconstruction metrics
+size_t f3r_pc_index_workspace(int32_t n) { return n > 0 ? f3r::pc_index_workspace(n) : 0; }
+
+int f3r_pc_index_build(const void* pts, int32_t f64, int32_t n, void* index, size_t index_bytes, void* stream) {
+  if (!pts || !index) return fail("f3r_pc_index_build: null operand");
+  if (n <= 0) return fail("f3r_pc_index_build: bad size n=%d (must be >= 1)", n);
+  if (index_bytes < f3r::pc_index_workspace(n)) return fail("f3r_pc_index_build: index block too small");
+  if (reinterpret_cast<uintptr_t>(index) & 255) return fail("f3r_pc_index_build: index block not 256-byte aligned");
+  int launches = 0;
+  const cudaError_t e = f3r::launch_pc_index_build(pts, f64 != 0, n, index, static_cast<cudaStream_t>(stream), &launches);
+  g_launches += launches;
+  return check(e, "f3r_pc_index_build");
+}
+
+size_t f3r_pc_query_workspace(int32_t nq) { return nq > 0 ? f3r::pc_query_workspace(nq) : 0; }
+
+int f3r_pc_nearest(const void* index, size_t index_bytes, int32_t n_ref, const void* query, int32_t f64, int32_t nq,
+                   double* dist, int64_t* idx, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!query || !dist || !idx) return fail("f3r_pc_nearest: null operand");
+  if (n_ref < 0 || nq <= 0) return fail("f3r_pc_nearest: bad sizes n_ref=%d nq=%d", n_ref, nq);
+  if (n_ref > 0) {
+    if (!index || !workspace) return fail("f3r_pc_nearest: null operand");
+    if (index_bytes < f3r::pc_index_workspace(n_ref)) return fail("f3r_pc_nearest: index block too small");
+    if (workspace_bytes < f3r::pc_query_workspace(nq)) return fail("f3r_pc_nearest: workspace too small");
+    if ((reinterpret_cast<uintptr_t>(index) | reinterpret_cast<uintptr_t>(workspace)) & 255)
+      return fail("f3r_pc_nearest: index or workspace not 256-byte aligned");
+  }
+  int launches = 0;
+  const cudaError_t e = f3r::launch_pc_nearest(index, n_ref, query, f64 != 0, nq, dist, reinterpret_cast<long long*>(idx),
+                                               workspace, static_cast<cudaStream_t>(stream), &launches);
+  g_launches += launches;
+  return check(e, "f3r_pc_nearest");
+}
+
+int f3r_pc_knn_normals(const void* index, size_t index_bytes, int32_t n, int32_t k, double* normals, void* stream) {
+  if (!index || !normals) return fail("f3r_pc_knn_normals: null operand");
+  if (n <= 0) return fail("f3r_pc_knn_normals: bad size n=%d", n);
+  if (k < 1 || k > 32) return fail("f3r_pc_knn_normals: k=%d must be in [1, 32]", k);
+  if (index_bytes < f3r::pc_index_workspace(n)) return fail("f3r_pc_knn_normals: index block too small");
+  if (reinterpret_cast<uintptr_t>(index) & 255) return fail("f3r_pc_knn_normals: index block not 256-byte aligned");
+  g_launches++;
+  return check(f3r::launch_pc_knn_normals(index, n, k, normals, static_cast<cudaStream_t>(stream)), "f3r_pc_knn_normals");
+}
+
+int f3r_pc_count_nonfinite(const void* pts, int32_t f64, int32_t n, uint32_t* count, void* stream) {
+  if (!count || (!pts && n)) return fail("f3r_pc_count_nonfinite: null operand");
+  if (n < 0) return fail("f3r_pc_count_nonfinite: bad size n=%d", n);
+  g_launches++;
+  return check(f3r::launch_pc_count_nonfinite(pts, f64 != 0, n, count, static_cast<cudaStream_t>(stream)),
+               "f3r_pc_count_nonfinite");
+}
+
+int f3r_pc_abs_dot(const double* a, const int64_t* a_idx, const double* b, const int64_t* b_idx, int32_t n, double* out,
+                   void* stream) {
+  if (!a || !b || !out) return fail("f3r_pc_abs_dot: null operand");
+  if (n < 0) return fail("f3r_pc_abs_dot: bad size n=%d", n);
+  g_launches++;
+  return check(f3r::launch_pc_abs_dot(a, reinterpret_cast<const long long*>(a_idx), b,
+                                      reinterpret_cast<const long long*>(b_idx), n, out, static_cast<cudaStream_t>(stream)),
+               "f3r_pc_abs_dot");
+}
+
+size_t f3r_f64_reduce_workspace(void) { return f3r::f64_reduce_workspace(); }
+
+static int reduce_args(const char* what, const double* x, int32_t n, const double* out, const void* workspace,
+                       size_t workspace_bytes) {
+  if (!x || !out || !workspace) return fail("%s: null operand", what);
+  if (n <= 0) return fail("%s: bad size n=%d (must be >= 1)", what, n);
+  if (workspace_bytes < f3r::f64_reduce_workspace()) return fail("%s: workspace too small", what);
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("%s: workspace not 256-byte aligned", what);
+  return 0;
+}
+
+int f3r_f64_mean(const double* x, int32_t n, double* out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (reduce_args("f3r_f64_mean", x, n, out, workspace, workspace_bytes)) return 1;
+  g_launches += 2;
+  return check(f3r::launch_f64_mean(x, n, out, workspace, static_cast<cudaStream_t>(stream)), "f3r_f64_mean");
+}
+
+int f3r_f64_median(const double* x, int32_t n, double* out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (reduce_args("f3r_f64_median", x, n, out, workspace, workspace_bytes)) return 1;
+  int launches = 0;
+  const cudaError_t e = f3r::launch_f64_median(x, n, out, workspace, static_cast<cudaStream_t>(stream), &launches);
+  g_launches += launches;
+  return check(e, "f3r_f64_median");
+}
+
+int f3r_f64_count_below(const double* x, int32_t n, const double* th, uint64_t* count, void* stream) {
+  if (!th || !count || (!x && n)) return fail("f3r_f64_count_below: null operand");
+  if (n < 0) return fail("f3r_f64_count_below: bad size n=%d", n);
+  g_launches++;
+  return check(f3r::launch_f64_count_below(x, n, th, reinterpret_cast<unsigned long long*>(count),
+                                           static_cast<cudaStream_t>(stream)), "f3r_f64_count_below");
+}
+
 // ---------------------------------------------------------------- block-level entry points
 size_t f3r_transformer_workspace(int32_t rows, int32_t dim, int32_t hidden) {
   // h [rows, dim] | q [rows, dim] | kv [rows, 2 dim] | att [rows, dim] | hid [rows, hidden], bf16, 256-byte aligned parts

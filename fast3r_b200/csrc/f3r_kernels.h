@@ -115,4 +115,20 @@ size_t focal_workspace(int views);
 cudaError_t launch_focal_weiszfeld(const float* pts, const float* conf, const float* thr, const float* pp, int views,
                                    int H, int W, int iters, float* focal, double* workspace, cudaStream_t stream);
 
+// reconstruction metrics (pointcloud.cu)
+size_t pc_index_workspace(int n);
+size_t pc_query_workspace(int nq);
+size_t f64_reduce_workspace();
+cudaError_t launch_pc_index_build(const void* pts, int f64, int n, void* index, cudaStream_t stream, int* launches);
+cudaError_t launch_pc_nearest(const void* index, int n_ref, const void* query, int f64, int nq, double* dist,
+                              long long* idx, void* workspace, cudaStream_t stream, int* launches);
+cudaError_t launch_pc_knn_normals(const void* index, int n, int k, double* normals, cudaStream_t stream);
+cudaError_t launch_pc_count_nonfinite(const void* pts, int f64, int n, unsigned int* count, cudaStream_t stream);
+cudaError_t launch_pc_abs_dot(const double* a, const long long* a_idx, const double* b, const long long* b_idx, int n,
+                              double* out, cudaStream_t stream);
+cudaError_t launch_f64_mean(const double* x, int n, double* out, void* workspace, cudaStream_t stream);
+cudaError_t launch_f64_median(const double* x, int n, double* out, void* workspace, cudaStream_t stream, int* launches);
+cudaError_t launch_f64_count_below(const double* x, int n, const double* th, unsigned long long* count,
+                                   cudaStream_t stream);
+
 }  // namespace f3r

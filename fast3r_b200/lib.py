@@ -90,6 +90,17 @@ _API = {
     "f3r_add_f32": (C.c_int, [_P, _P, _SIZE, _P]),
     "f3r_attention_x3_workspace": (_SIZE, [_I32, _I32, _I32, _I32]),
     "f3r_attention_x3": (C.c_int, [_P, _I32, _P, _I32, _P, _I32, _P, _P, _SIZE, _I32, _I32, _I32, _I32, _F32, _P]),
+    "f3r_pc_index_workspace": (_SIZE, [_I32]),
+    "f3r_pc_index_build": (C.c_int, [_P, _I32, _I32, _P, _SIZE, _P]),
+    "f3r_pc_query_workspace": (_SIZE, [_I32]),
+    "f3r_pc_nearest": (C.c_int, [_P, _SIZE, _I32, _P, _I32, _I32, _P, _P, _P, _SIZE, _P]),
+    "f3r_pc_knn_normals": (C.c_int, [_P, _SIZE, _I32, _I32, _P, _P]),
+    "f3r_pc_count_nonfinite": (C.c_int, [_P, _I32, _I32, _P, _P]),
+    "f3r_pc_abs_dot": (C.c_int, [_P, _P, _P, _P, _I32, _P, _P]),
+    "f3r_f64_reduce_workspace": (_SIZE, []),
+    "f3r_f64_mean": (C.c_int, [_P, _I32, _P, _P, _SIZE, _P]),
+    "f3r_f64_median": (C.c_int, [_P, _I32, _P, _P, _SIZE, _P]),
+    "f3r_f64_count_below": (C.c_int, [_P, _I32, _P, _P, _P]),
 }
 EXPORTS = list(_API)
 

@@ -339,3 +339,109 @@ def focal_weiszfeld(pts: torch.Tensor, conf: Optional[torch.Tensor] = None, thr:
     _call("f3r_focal_weiszfeld", pts, _ptr(pts), _ptr(conf), _ptr(thr), _ptr(pp), views, h, w, int(iters), _ptr(focal),
           _ptr(ws), nbytes)
     return focal
+
+
+# ------------------------------------------------------------------ reconstruction metrics (csrc/pointcloud.cu)
+F64 = torch.float64
+
+
+def _points(x: torch.Tensor, name: str) -> int:
+    if x.dtype not in (F32, F64):
+        raise TypeError(f"{name}: expected float32 or float64, got {x.dtype}")
+    if x.dim() != 2 or x.shape[1] != 3:
+        raise ValueError(f"{name}: expected shape (n, 3), got {tuple(x.shape)}")
+    if not x.is_contiguous():
+        raise ValueError(f"{name}: must be contiguous")
+    return int(x.dtype == F64)
+
+
+class PointIndex:
+    """Spatial index over a point cloud (f3r_pc_index_build): the caller-owned block and the cloud's size."""
+
+    def __init__(self, block: Optional[torch.Tensor], n: int, device: torch.device):
+        self.block, self.n, self.device = block, n, device
+
+
+def pc_index(pts: torch.Tensor) -> PointIndex:
+    """pts float32 / float64 (n, 3) on the device -> PointIndex (n == 0: an empty index that no query matches)."""
+    f64 = _points(pts, "pts")
+    n = pts.shape[0]
+    if n == 0:
+        return PointIndex(None, 0, pts.device)
+    nbytes = L.load().f3r_pc_index_workspace(n)
+    block = _scratch(nbytes, pts.device)
+    _call("f3r_pc_index_build", pts, _ptr(pts), f64, n, _ptr(block), nbytes)
+    return PointIndex(block, n, pts.device)
+
+
+def pc_nearest(index: PointIndex, query: torch.Tensor):
+    """Exact nearest indexed point of every query point: (dist float64 (nq,), idx int64 (nq,)), as cKDTree.query."""
+    f64 = _points(query, "query")
+    nq = query.shape[0]
+    dist = torch.empty(nq, dtype=F64, device=query.device)
+    idx = torch.empty(nq, dtype=torch.int64, device=query.device)
+    if nq == 0:
+        return dist, idx
+    nbytes = L.load().f3r_pc_query_workspace(nq) if index.n else 0
+    ws = _scratch(nbytes, query.device) if nbytes else None
+    block = index.block
+    _call("f3r_pc_nearest", query, _ptr(block), block.numel() if block is not None else 0, index.n, _ptr(query), f64, nq,
+          _ptr(dist), _ptr(idx), _ptr(ws), nbytes)
+    return dist, idx
+
+
+def pc_knn_normals(index: PointIndex, k: int = 30) -> torch.Tensor:
+    """float64 (n, 3) unit normals of the indexed cloud from its k nearest points (the point included)."""
+    out = torch.empty(index.n, 3, dtype=F64, device=index.device)
+    if index.n:
+        _call("f3r_pc_knn_normals", out, _ptr(index.block), index.block.numel(), index.n, int(k), _ptr(out))
+    return out
+
+
+def pc_count_nonfinite(pts: torch.Tensor) -> torch.Tensor:
+    """Number of non-finite coordinates of pts (n, 3), as a device int32 (1,) tensor."""
+    f64 = _points(pts, "pts")
+    count = torch.empty(1, dtype=torch.int32, device=pts.device)
+    _call("f3r_pc_count_nonfinite", pts, _ptr(pts), f64, pts.shape[0], _ptr(count))
+    return count
+
+
+def pc_abs_dot(a: torch.Tensor, b: torch.Tensor, a_idx: Optional[torch.Tensor] = None,
+               b_idx: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """|a[a_idx] . b[b_idx]| row by row (float64 (.., 3); int64 indices or None for the identity)."""
+    _chk(a, F64, "a"); _chk(b, F64, "b")
+    for t, name in ((a_idx, "a_idx"), (b_idx, "b_idx")):
+        if t is not None:
+            _chk(t, torch.int64, name)
+    n = (a_idx if a_idx is not None else b_idx if b_idx is not None else a).shape[0]
+    out = torch.empty(n, dtype=F64, device=a.device)
+    _call("f3r_pc_abs_dot", out, _ptr(a), _ptr(a_idx), _ptr(b), _ptr(b_idx), n, _ptr(out))
+    return out
+
+
+def _reduce(name: str, x: torch.Tensor) -> torch.Tensor:
+    _chk(x, F64, "x")
+    nbytes = L.load().f3r_f64_reduce_workspace()
+    ws = _scratch(nbytes, x.device)
+    out = torch.empty((), dtype=F64, device=x.device)
+    _call(name, x, _ptr(x), x.numel(), _ptr(out), _ptr(ws), nbytes)
+    return out
+
+
+def f64_mean(x: torch.Tensor) -> torch.Tensor:
+    """Mean of a float64 tensor (n >= 1) in a fixed summation order, as a 0-d device tensor."""
+    return _reduce("f3r_f64_mean", x)
+
+
+def f64_median(x: torch.Tensor) -> torch.Tensor:
+    """numpy.median of a float64 tensor (n >= 1), exactly, as a 0-d device tensor."""
+    return _reduce("f3r_f64_median", x)
+
+
+def f64_count_below(x: torch.Tensor, th: float) -> torch.Tensor:
+    """Number of elements of a float64 tensor that are < th, as a device int64 (1,) tensor."""
+    _chk(x, F64, "x")
+    t = torch.tensor([float(th)], dtype=F64, device=x.device)
+    count = torch.empty(1, dtype=torch.int64, device=x.device)
+    _call("f3r_f64_count_below", x, _ptr(x), x.numel(), _ptr(t), _ptr(count))
+    return count

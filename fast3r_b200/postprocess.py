@@ -10,6 +10,8 @@ Same names, arguments and results as the reference:
 * ``estimate_focal(pts3d_i, conf_i, pp=None, min_conf_thr_percentile=10)`` - multiview_dust3r_module.py:1081-1109
   (returns a python float), and ``estimate_focal_knowing_depth(pts3d, pp, focal_mode="weiszfeld")`` -
   fast3r/dust3r/post_process.py:19-79 (returns a (B,) tensor).
+* ``evaluate_reconstruction(views, preds, ...)`` - MultiViewDUSt3RLitModule.evaluate_reconstruction
+  (multiview_dust3r_module.py:551-735): registration, normals and the metrics of fast3r_b200.recon_metric per batch item.
 
 NOT here (documented in DESIGN.md §1): fast_pnp / cv2.solvePnPRansac (cloud_opt/init_im_poses.py:300-350) and the
 "median" focal mode.  Tensors may live on the CPU (what ``inference()`` returns) or on a CUDA device; CPU inputs are
@@ -103,3 +105,65 @@ def estimate_focal_knowing_depth(pts3d: torch.Tensor, pp: torch.Tensor, focal_mo
     dev = _device_of(pts3d, device)
     ppt = _f32(torch.as_tensor(pp), dev).reshape(-1, 2).expand(b, 2).contiguous()
     return ops.focal_weiszfeld(_f32(pts3d, dev), None, None, ppt, iters=10).to(pts3d.device)
+
+
+def evaluate_reconstruction(views: List[Dict], preds: List[Dict], min_conf_thr_percentile_for_local_alignment_and_icp=0,
+                            min_conf_thr_percentile_for_metric_cacluation=0, use_pts3d_from_local_head=True,
+                            device=None) -> List[Dict]:
+    """MultiViewDUSt3RLitModule.evaluate_reconstruction (multiview_dust3r_module.py:551-735) on the GPU, without the
+    Lightning side: returns one ``{scene_name: {accuracy, accuracy_median, completion, completion_median, nc1,
+    nc1_median, nc2, nc2_median}}`` per batch item instead of accumulating them in the module.
+
+    Per item: per-view quantile masks, the similarity of the masked predicted points onto the ground truth over all views
+    at once (the boolean-weighted roma.rigid_points_registration is Umeyama over the points of weight 1), Open3D-style
+    k=30 normals of both clouds, then accuracy / completion / normal consistency (fast3r_b200.recon_metric).  One
+    difference: with fewer than 3 registration points the fit returns the identity (the fallback of similarity_fit);
+    roma has no such fallback."""
+    from . import recon_metric as rm
+    if use_pts3d_from_local_head:
+        align_local_pts3d_to_global(preds, views, min_conf_thr_percentile=min_conf_thr_percentile_for_local_alignment_and_icp,
+                                    device=device)
+    assert min_conf_thr_percentile_for_local_alignment_and_icp >= min_conf_thr_percentile_for_metric_cacluation
+    if not views:
+        return []
+    dev = _device_of(preds[0]["pts3d_in_other_view"], device)
+    results = []
+    for i in range(len(views[0]["img"])):
+        # the reference names the scene after views[i] (the view with the item's index), kept as is
+        scene_name = "/".join(views[i]["label"][0].split("/")[:-1]) if "label" in views[i] else "unknown"
+        pred_aligned, gt_pts, _ = _registered_clouds(views, preds, i, min_conf_thr_percentile_for_local_alignment_and_icp,
+                                                      min_conf_thr_percentile_for_metric_cacluation,
+                                                      use_pts3d_from_local_head, dev)
+        pred_normals = rm.estimate_normals(pred_aligned)
+        gt_normals = rm.estimate_normals(gt_pts)
+        acc, acc_med, nc1, nc1_med = rm.accuracy(gt_pts, pred_aligned, gt_normals, pred_normals)
+        comp, comp_med, nc2, nc2_med = rm.completion(gt_pts, pred_aligned, gt_normals, pred_normals)
+        results.append({scene_name: {
+            "accuracy": acc, "accuracy_median": acc_med, "completion": comp, "completion_median": comp_med,
+            "nc1": nc1, "nc1_median": nc1_med, "nc2": nc2, "nc2_median": nc2_med,
+        }})
+    return results
+
+
+def _registered_clouds(views, preds, i: int, pct_icp: float, pct_metric: float, use_local: bool, dev: torch.device):
+    """Batch item i of evaluate_reconstruction up to the metrics (multiview_dust3r_module.py:565-660): the predicted
+    points with valid & conf >= quantile(pct_metric) of their view, registered onto the ground truth by the similarity
+    fitted over those of them that also pass quantile(pct_icp); and all valid ground-truth points.  Returns
+    (pred_aligned fp32 (m, 3), gt fp32 (g, 3), rts fp32 (13,)), points view-major in raster order as the reference
+    concatenates them."""
+    key_pts, key_conf = ("pts3d_local_aligned_to_global", "conf_local") if use_local else ("pts3d_in_other_view", "conf")
+    x = torch.stack([_f32(p[key_pts][i], dev) for p in preds])              # (V, H, W, 3)
+    conf = torch.stack([_f32(p[key_conf][i], dev) for p in preds])          # (V, H, W)
+    y = torch.stack([_f32(v["pts3d"][i], dev) for v in views])
+    valid = torch.stack([v["valid_mask"][i].to(dev, torch.bool) for v in views])
+    nv = x.shape[0]
+    n = x[0, ..., 0].numel()
+    conf_v = conf.reshape(nv, n).contiguous()
+    thr_metric = ops.conf_quantile(conf_v, float(pct_metric) / 100.0)
+    thr_icp = ops.conf_quantile(conf_v, float(pct_icp) / 100.0)
+    mask_pred = valid.reshape(nv, n) & (conf_v >= thr_metric[:, None])
+    weights = mask_pred & (conf_v >= thr_icp[:, None])
+    xs, ys = x.reshape(1, nv * n, 3).contiguous(), y.reshape(1, nv * n, 3).contiguous()
+    rts = ops.similarity_fit(xs, ys, None, None, weights.reshape(1, nv * n).to(torch.uint8).contiguous())
+    aligned = ops.similarity_apply(xs, rts)[0]
+    return aligned[mask_pred.reshape(-1)].contiguous(), y[valid].contiguous(), rts[0]

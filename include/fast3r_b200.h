@@ -222,6 +222,44 @@ int f3r_attention_x3(const float* q, int32_t ldq, const float* kv, int32_t ldkv,
                      void* workspace, size_t workspace_bytes, int32_t batch, int32_t heads, int32_t sq, int32_t skv,
                      float scale, void* stream);
 
+/* ---- reconstruction metrics: accuracy / completion / completion_ratio of fast3r/eval/recon_metric.py:14-49 and the
+ * normals of evaluate_reconstruction (fast3r/models/multiview_dust3r_module.py:551-735), exact with respect to scipy's
+ * cKDTree.  Point clouds are DEVICE arrays [n][3] of fp32 (f64 == 0) or fp64 (f64 != 0), converted exactly to fp64.
+ * Coordinates must be finite (check with the non-finite count first): a non-finite point never faults, but it makes
+ * the search exhaustive and its results are unspecified.
+ *
+ * Spatial index over a reference cloud of n >= 1 points, built into a caller-owned block of
+ *   f3r_pc_index_workspace(n) bytes, 256-byte aligned: Morton order (radix sort), buckets of 32 consecutive points with
+ *   fp64 bounding boxes, parents of 8 consecutive children.  The block also holds the build's scratch; it stays valid
+ *   until the caller reuses it.
+ * Nearest: for each of nq query points the exact nearest reference point under scipy's arithmetic,
+ *   dist (fp64) = sqrt((dx*dx + dy*dy) + dz*dz) and idx (int64, original index; any one of equidistant points).
+ *   n_ref == 0 (index may be NULL): dist = +inf, idx = n_ref, as scipy.  workspace: f3r_pc_query_workspace(nq) bytes,
+ *   256-byte aligned (the queries are processed in Morton order).
+ * kNN normals of the indexed cloud itself: per point the unit eigenvector of the smallest eigenvalue of the fp64
+ *   covariance of its k <= 32 nearest points, the point included (Open3D's EstimateNormals with KDTreeSearchParamKNN);
+ *   fewer than 3 points: (0, 0, 1).  The sign is unspecified.  normals fp64 [n][3], original order.
+ * Non-finite count: *count (device uint32) = number of non-finite coordinates of the n points.
+ * Absolute dot: out[i] = |a[ia] . b[ib]| (ia = a_idx[i], or i when a_idx is NULL; int64 indices), rounded as numpy's
+ *   np.abs(np.sum(a * b, axis=-1)).
+ * fp64 reductions over x[0..n): mean in a fixed order (not numpy's pairwise order: equal to a few ulp), median exactly
+ *   as numpy.median (radix select on the bit patterns; the mean of the two middle values for even n), and the count
+ *   of x < *th (th a device fp64 scalar) into *count (device uint64).  workspace: f3r_f64_reduce_workspace() bytes,
+ *   256-byte aligned. */
+size_t f3r_pc_index_workspace(int32_t n);
+int f3r_pc_index_build(const void* pts, int32_t f64, int32_t n, void* index, size_t index_bytes, void* stream);
+size_t f3r_pc_query_workspace(int32_t nq);
+int f3r_pc_nearest(const void* index, size_t index_bytes, int32_t n_ref, const void* query, int32_t f64, int32_t nq,
+                   double* dist, int64_t* idx, void* workspace, size_t workspace_bytes, void* stream);
+int f3r_pc_knn_normals(const void* index, size_t index_bytes, int32_t n, int32_t k, double* normals, void* stream);
+int f3r_pc_count_nonfinite(const void* pts, int32_t f64, int32_t n, uint32_t* count, void* stream);
+int f3r_pc_abs_dot(const double* a, const int64_t* a_idx, const double* b, const int64_t* b_idx, int32_t n, double* out,
+                   void* stream);
+size_t f3r_f64_reduce_workspace(void);
+int f3r_f64_mean(const double* x, int32_t n, double* out, void* workspace, size_t workspace_bytes, void* stream);
+int f3r_f64_median(const double* x, int32_t n, double* out, void* workspace, size_t workspace_bytes, void* stream);
+int f3r_f64_count_below(const double* x, int32_t n, const double* th, uint64_t* count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
