@@ -562,63 +562,6 @@ int f3r_f64_count_below(const double* x, int32_t n, const double* th, uint64_t* 
                                            static_cast<cudaStream_t>(stream)), "f3r_f64_count_below");
 }
 
-// ---------------------------------------------------------------- block-level entry points
-size_t f3r_transformer_workspace(int32_t rows, int32_t dim, int32_t hidden) {
-  // h [rows, dim] | q [rows, dim] | kv [rows, 2 dim] | att [rows, dim] | hid [rows, hidden], bf16, 256-byte aligned parts
-  auto al = [](size_t b) { return (b + 255) & ~static_cast<size_t>(255); };
-  const size_t r = static_cast<size_t>(rows);
-  return 3 * al(r * dim * 2) + al(r * 2 * dim * 2) + al(r * hidden * 2);
-}
-
-int f3r_transformer_blocks(const f3r_block_weights* blocks, int32_t n_blocks, float* x, int32_t batch, int32_t seq,
-                           int32_t dim, int32_t heads, int32_t hidden, float eps, float scale, int32_t rope_grid_w,
-                           int32_t rope_tok_per_img, const float* rope_cos, const float* rope_sin, void* workspace,
-                           size_t workspace_bytes, void* stream) {
-  if (!blocks || n_blocks <= 0 || !x || !workspace) return fail("f3r_transformer_blocks: null operand");
-  if (batch <= 0 || seq <= 0 || dim != heads * 64 || hidden <= 0) return fail("f3r_transformer_blocks: bad shape (head_dim must be 64)");
-  const int32_t rows = batch * seq;
-  if (workspace_bytes < f3r_transformer_workspace(rows, dim, hidden)) return fail("f3r_transformer_blocks: workspace too small");
-  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("f3r_transformer_blocks: workspace not 256-byte aligned");
-  auto al = [](size_t b) { return (b + 255) & ~static_cast<size_t>(255); };
-  uint8_t* w = static_cast<uint8_t*>(workspace);
-  const size_t r = static_cast<size_t>(rows);
-  void* h = w;
-  void* q = w + al(r * dim * 2);
-  void* kv = static_cast<uint8_t*>(q) + al(r * dim * 2);
-  void* att = static_cast<uint8_t*>(kv) + al(r * 2 * dim * 2);
-  void* hid = static_cast<uint8_t*>(att) + al(r * dim * 2);
-  const bool rope = rope_cos != nullptr;
-  for (int i = 0; i < n_blocks; ++i) {
-    const f3r_block_weights& b = blocks[i];
-    // x += proj(attention(rope(q), rope(k), v));  x += fc2(gelu(fc1(LN(x))))     (fast3r/croco/models/blocks.py:236-239)
-    if (f3r_layernorm(x, b.norm1_w, b.norm1_b, h, 0, rows, dim, eps, stream)) return 1;
-    f3r_gemm_desc d;
-    memset(&d, 0, sizeof(d));
-    d.a = h; d.wt = b.qkv_w; d.n = 3 * dim; d.k = dim; d.taps = 1; d.w = rows; d.h = 1; d.nb = 1; d.a_ld = dim;
-    d.bias = b.qkv_b; d.out0 = q; d.ldo = dim; d.split_col = dim; d.out0b = kv; d.ldo_b = 2 * dim;
-    if (rope) {
-      d.epi = F3R_EPI_ROPE; d.tok_per_img = rope_tok_per_img; d.grid_w = rope_grid_w; d.rope_cols = 2 * dim;
-      d.rope_cos = rope_cos; d.rope_sin = rope_sin;
-    }
-    if (f3r_gemm(&d, stream)) return 1;
-    if (f3r_attention(q, dim, kv, 2 * dim, att, dim, nullptr, batch, heads, seq, seq, scale, stream)) return 1;
-    memset(&d, 0, sizeof(d));
-    d.a = att; d.wt = b.proj_w; d.n = dim; d.k = dim; d.taps = 1; d.w = rows; d.h = 1; d.nb = 1; d.a_ld = dim;
-    d.bias = b.proj_b; d.out0 = x; d.out0_f32 = 1; d.res0 = x; d.res0_f32 = 1; d.ldo = dim;
-    if (f3r_gemm(&d, stream)) return 1;
-    if (f3r_layernorm(x, b.norm2_w, b.norm2_b, h, 0, rows, dim, eps, stream)) return 1;
-    memset(&d, 0, sizeof(d));
-    d.a = h; d.wt = b.fc1_w; d.n = hidden; d.k = dim; d.taps = 1; d.w = rows; d.h = 1; d.nb = 1; d.a_ld = dim;
-    d.bias = b.fc1_b; d.out0 = hid; d.ldo = hidden; d.act = F3R_ACT_GELU;
-    if (f3r_gemm(&d, stream)) return 1;
-    memset(&d, 0, sizeof(d));
-    d.a = hid; d.wt = b.fc2_w; d.n = dim; d.k = hidden; d.taps = 1; d.w = rows; d.h = 1; d.nb = 1; d.a_ld = hidden;
-    d.bias = b.fc2_b; d.out0 = x; d.out0_f32 = 1; d.res0 = x; d.res0_f32 = 1; d.ldo = dim;
-    if (f3r_gemm(&d, stream)) return 1;
-  }
-  return 0;
-}
-
 int f3r_cast_bf16(const float* in, void* out, size_t count, void* stream) {
   if (!in || !out) return fail("f3r_cast_bf16: null operand");
   g_launches++;

@@ -36,10 +36,7 @@ class GemmDesc(C.Structure):
     ]
 
 
-ABI_VERSION = 2
-class BlockWeights(C.Structure):
-    _fields_ = [(n, C.c_void_p) for n in ("norm1_w", "norm1_b", "norm2_w", "norm2_b", "qkv_w", "qkv_b", "proj_w", "proj_b",
-                                          "fc1_w", "fc1_b", "fc2_w", "fc2_b")]
+ABI_VERSION = 3
 
 
 JPEG_SUPPORTED, JPEG_UNSUPPORTED, JPEG_MALFORMED = range(3)
@@ -71,9 +68,6 @@ _API = {
     "f3r_im2col3x3s2": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "f3r_upsample2x": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "f3r_cast_bf16": (C.c_int, [_P, _P, _SIZE, _P]),
-    "f3r_transformer_workspace": (_SIZE, [_I32, _I32, _I32]),
-    "f3r_transformer_blocks": (C.c_int, [C.POINTER(BlockWeights), _I32, _P, _I32, _I32, _I32, _I32, _I32, _F32, _F32,
-                                         _I32, _I32, _P, _P, _P, _SIZE, _P]),
     "f3r_resample_ksize": (C.c_int, [_I32, _I32, _I32]),
     "f3r_resample_coeffs": (C.c_int, [_I32, _I32, _I32, _P, _P]),
     "f3r_ingest_rgb8": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _I32, _I32, _P, _P, _I32, _P, _I32, _I32, _I32,

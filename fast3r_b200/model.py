@@ -24,7 +24,6 @@ import torch.nn as nn
 
 from . import lib as L
 from . import ops
-from .ops import attention_units  # host arithmetic, not a library call: stays real when `ops` is replaced
 
 try:  # same hub integration as the reference (fast3r/models/fast3r.py:45-49): from_pretrained / save_pretrained
     from huggingface_hub import PyTorchModelHubMixin as _HubMixin
@@ -500,14 +499,9 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
             x = torch.empty(M, D, dtype=F32, device=imgs.device)
             P_.linear(a0, P_.pe_w, P_.pe_b, out0=x)
             self._tap("patch_embed", x)
-            if not P_.x3 and self._taps is None and ops.pick_kv_split(attention_units(c, enc.num_heads, P), (P + 127) // 128) == 1:
-                # all encoder blocks of this chunk in ONE library call (f3r_transformer_blocks: the same seven launches per
-                # block, issued by the C side with its own workspace carving)
-                ops.transformer_blocks(x, P_.enc, batch=c, seq=P, heads=enc.num_heads, eps=1e-6, scale=64 ** -0.5, rope=rope)
-            else:
-                for li, w in enumerate(P_.enc):
-                    self._block(x, w, ws, batch=c, seq=P, heads=enc.num_heads, eps=1e-6, scale=64 ** -0.5, rope=rope)
-                    self._tap(f"enc_block{li}", x)
+            for li, w in enumerate(P_.enc):
+                self._block(x, w, ws, batch=c, seq=P, heads=enc.num_heads, eps=1e-6, scale=64 ** -0.5, rope=rope)
+                self._tap(f"enc_block{li}", x)
             ops.layernorm(x, P_.enc_nw, P_.enc_nb, 1e-6, feats[s * P:(s + c) * P])
         return feats, P, gh, gw
 

@@ -219,29 +219,6 @@ def attention_x3(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch:
           sq, skv, float(scale))
 
 
-def transformer_blocks(x: torch.Tensor, blocks, *, batch: int, seq: int, heads: int, eps: float, scale: float,
-                       rope=None):
-    """n consecutive transformer blocks on the fp32 residual stream x (batch*seq, D), in place, in ONE library call
-    (f3r_transformer_blocks).  `blocks`: objects with n1w, n1b, n2w, n2b, qkv_w, qkv_b, proj_w, proj_b, fc1_w, fc1_b,
-    fc2_w, fc2_b (bf16 weights [N, 1, K], fp32 biases); rope: dict(P=tokens per image, gw=grid width, cos=, sin=) or None."""
-    _chk(x, F32, "x")
-    D = x.shape[-1]
-    hidden = blocks[0].fc1_w.shape[0]
-    arr = (L.BlockWeights * len(blocks))()
-    for i, b in enumerate(blocks):
-        for name, t in (("norm1_w", b.n1w), ("norm1_b", b.n1b), ("norm2_w", b.n2w), ("norm2_b", b.n2b),
-                        ("qkv_w", b.qkv_w), ("qkv_b", b.qkv_b), ("proj_w", b.proj_w), ("proj_b", b.proj_b),
-                        ("fc1_w", b.fc1_w), ("fc1_b", b.fc1_b), ("fc2_w", b.fc2_w), ("fc2_b", b.fc2_b)):
-            setattr(arr[i], name, _ptr(t))
-    rows = batch * seq
-    assert x.numel() == rows * D
-    nbytes = L.load().f3r_transformer_workspace(rows, D, hidden)
-    ws = _scratch(nbytes, x.device)
-    _call("f3r_transformer_blocks", x, arr, len(blocks), _ptr(x), batch, seq, D, heads, hidden, float(eps), float(scale),
-          rope["gw"] if rope else 0, rope["P"] if rope else 0, _ptr(rope["cos"]) if rope else None,
-          _ptr(rope["sin"]) if rope else None, _ptr(ws), nbytes)
-
-
 def layernorm(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float, out: torch.Tensor):
     _chk(x, F32, "x"); _chk(w, F32, "w"); _chk(b, F32, "b")
     assert out.dtype in (BF16, F32) and out.is_contiguous() and out.numel() == x.numel()

@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define F3R_ABI_VERSION 2
+#define F3R_ABI_VERSION 3
 
 /* epilogue kinds of f3r_gemm */
 enum { F3R_EPI_STORE = 0, F3R_EPI_ROPE = 1, F3R_EPI_IDXEMB = 2, F3R_EPI_CONVT = 3, F3R_EPI_FINAL = 4 };
@@ -118,26 +118,6 @@ int f3r_upsample2x(const void* in, void* out, int32_t f32, int32_t n, int32_t h,
                    int32_t wo, void* stream);
 /* fp32 -> bf16, count multiple of 4 */
 int f3r_cast_bf16(const float* in, void* out, size_t count, void* stream);
-
-
-/* ---- block-level entry: n_blocks consecutive transformer blocks (fast3r/croco/models/blocks.py:197-239) on the fp32
- * residual stream x [batch*seq, dim], in place:  x += proj(SDPA(rope(q), rope(k), v));  x += fc2(GELU(fc1(LN(x)))).
- * Composition of f3r_layernorm / f3r_gemm / f3r_attention (7 launches per block) with the operand buffers carved out of a
- * caller-owned workspace (f3r_transformer_workspace bytes, 256-byte aligned) - a C / C++ caller runs the CroCo encoder
- * (rope_cos != NULL: RoPE2D on q, k with positions from the patch grid) or a span of fusion-decoder blocks (rope_cos ==
- * NULL) with one call.  bf16 fast path, single device; attention over all seq keys of each batch element. */
-typedef struct f3r_block_weights {
-  const float* norm1_w; const float* norm1_b; const float* norm2_w; const float* norm2_b;   /* fp32 [dim]           */
-  const void* qkv_w;  const float* qkv_b;   /* bf16 [3 dim, dim] rows ordered q | k | v (blocks.py:138-143), fp32 [3 dim] */
-  const void* proj_w; const float* proj_b;  /* bf16 [dim, dim], fp32 [dim]                                           */
-  const void* fc1_w;  const float* fc1_b;   /* bf16 [hidden, dim], fp32 [hidden]                                     */
-  const void* fc2_w;  const float* fc2_b;   /* bf16 [dim, hidden], fp32 [dim]                                        */
-} f3r_block_weights;
-size_t f3r_transformer_workspace(int32_t rows, int32_t dim, int32_t hidden);
-int f3r_transformer_blocks(const f3r_block_weights* blocks, int32_t n_blocks, float* x, int32_t batch, int32_t seq,
-                           int32_t dim, int32_t heads, int32_t hidden, float eps, float scale, int32_t rope_grid_w,
-                           int32_t rope_tok_per_img, const float* rope_cos, const float* rope_sin, void* workspace,
-                           size_t workspace_bytes, void* stream);
 
 /* ---- image ingest (SURVEY §8 f3): PIL.Image.resize(LANCZOS | BICUBIC) + center crop + ToTensor + Normalize(0.5, 0.5) of
  * load_images() (fast3r/dust3r/utils/image.py:68-159) on a decoded 8-bit RGB image, bit-exact with Pillow's 8-bit

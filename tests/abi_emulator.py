@@ -164,27 +164,6 @@ def attention_merge(part_o, part_lse, n_parts, out, *, batch, heads, sq):
     _store(out, (o * w[..., None]).sum(0).reshape(batch * sq, heads * 64))
 
 
-def transformer_blocks(x, blocks, *, batch, seq, heads, eps, scale, rope=None):
-    """f3r_transformer_blocks = the per-op sequence of Fast3R._block, carried out by the library."""
-    M, D = x.shape
-    hidden = blocks[0].fc1_w.shape[0]
-    h, q, kv, att = (torch.empty(M, D, dtype=BF16) for _ in range(4))
-    kv = torch.empty(M, 2 * D, dtype=BF16)
-    hid = torch.empty(M, hidden, dtype=BF16)
-    for b in blocks:
-        layernorm(x, b.n1w, b.n1b, eps, h)
-        if rope is not None:
-            linear(h, b.qkv_w, b.qkv_b, out0=q, ldo=D, split_col=D, out0b=kv, ldo_b=2 * D, epi=L.EPI_ROPE,
-                   tok_per_img=rope["P"], grid_w=rope["gw"], rope_cols=2 * D, rope_cos=rope["cos"], rope_sin=rope["sin"])
-        else:
-            linear(h, b.qkv_w, b.qkv_b, out0=q, ldo=D, split_col=D, out0b=kv, ldo_b=2 * D)
-        attention(q, kv, att, batch=batch, heads=heads, sq=seq, skv=seq, scale=scale)
-        linear(att, b.proj_w, b.proj_b, out0=x, res0=x)
-        layernorm(x, b.n2w, b.n2b, eps, h)
-        linear(h, b.fc1_w, b.fc1_b, out0=hid, act=L.ACT_GELU)
-        linear(hid, b.fc2_w, b.fc2_b, out0=x, res0=x)
-
-
 def layernorm(x, w, b, eps, out):
     _store(out, F.layer_norm(x.float(), (x.shape[-1],), w.float(), b.float(), eps))
 

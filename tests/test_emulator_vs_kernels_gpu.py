@@ -144,33 +144,3 @@ def test_kernel_matches_emulator(name):
         if key in ("pts", "conf"):
             tol = 2e-3
         assert _rel(got, want) < tol, (name, key, _rel(got, want))
-
-
-def test_transformer_blocks_entry_equals_per_op_sequence():
-    """f3r_transformer_blocks (one C call for a span of blocks) must reproduce the per-op sequence bit for bit: encoder
-    flavour (RoPE) and decoder flavour (no RoPE, other eps / scale)."""
-    from fast3r_b200 import Fast3R, tiny_args, ops
-    from fast3r_b200.model import _BlockW
-    from tests.golden.synth import synth_state_dict
-    enc, dec, head = tiny_args()
-    model = Fast3R(enc, dec, head).eval()
-    shapes = {k: tuple(v.shape) for k, v in model.state_dict().items()}
-    model.load_state_dict(synth_state_dict(shapes, seed=0))
-    model = model.cuda()
-    D, heads, hidden = 128, 2, 512
-    gh, gw, n = 4, 6, 3
-    P = gh * gw
-    j = torch.arange(16, dtype=torch.float32)
-    ang = torch.arange(8, dtype=torch.float32)[:, None] * (1.0 / (100.0 ** (j / 16.0)))[None]
-    rope = dict(P=P, gw=gw, cos=ang.cos().contiguous().cuda(), sin=ang.sin().contiguous().cuda())
-    for blocks, rp, eps, scale, batch, seq in (
-            ([_BlockW(b) for b in model.encoder.enc_blocks], rope, 1e-6, 0.125, n, P),
-            ([_BlockW(b) for b in model.decoder.dec_blocks[:3]], None, 1e-5, 0.16019, 1, n * P)):
-        x0 = _r((batch * seq, D), 77, 1.0, torch.float32).cuda()
-        xa, xb = x0.clone(), x0.clone()
-        ops.transformer_blocks(xa, blocks, batch=batch, seq=seq, heads=heads, eps=eps, scale=scale, rope=rp)
-        ws = Fast3R._workspace(batch * seq, D, hidden, xb.device)
-        for w in blocks:
-            Fast3R._block(xb, w, ws, batch=batch, seq=seq, heads=heads, eps=eps, scale=scale, rope=rp)
-        torch.cuda.synchronize()
-        assert torch.equal(xa, xb)
