@@ -276,18 +276,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 }
 
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, cudaStream_t stream) {
-  // (set on every launch: the attribute is per device and one process may drive several GPUs)
-  cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM_BYTES);
-  if (e != cudaSuccess) return e;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(a.batch * a.heads * a.q_tiles * a.n_split);
-  cfg.blockDim = dim3(ATT_THREADS);
-  cfg.dynamicSmemBytes = ATT_SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  cfg.attrs = attr;
-  cfg.numAttrs = launch_attrs(attr, 1);
-  return cudaLaunchKernelEx(&cfg, attention_kernel, tq, tkv, a);
+  return launch(attention_kernel, a.batch * a.heads * a.q_tiles * a.n_split, ATT_THREADS, ATT_SMEM_BYTES, stream, true, tq,
+                tkv, a);
 }
 
 // ---------------------------------------------------------------- merge of key-slice partials
@@ -329,15 +319,8 @@ cudaError_t launch_attention_merge(const float* part_o, const float* part_lse, i
                                    void* out, int ldo, cudaStream_t stream) {
   const size_t total = static_cast<size_t>(batch) * sq * heads * 8;
   if (total == 0) return cudaSuccess;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>((total + 255) / 256));
-  cfg.blockDim = dim3(256);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  cfg.attrs = attr;
-  cfg.numAttrs = launch_attrs(attr, 1);
-  return cudaLaunchKernelEx(&cfg, attention_merge_kernel, part_o, part_lse, n_parts, batch, heads, sq,
-                            static_cast<__nv_bfloat16*>(out), ldo);
+  return launch(attention_merge_kernel, static_cast<unsigned>((total + 255) / 256), 256, 0, stream, true, part_o, part_lse,
+                n_parts, batch, heads, sq, static_cast<__nv_bfloat16*>(out), ldo);
 }
 
 }  // namespace f3r

@@ -181,11 +181,8 @@ attention_x3_kernel(const __grid_constant__ CUtensorMap tmap_q3, const __grid_co
 
 cudaError_t launch_attention_x3(const CUtensorMap& tq3, const CUtensorMap& tk3, const CUtensorMap& tv2,
                                 const AttnArgs& a, cudaStream_t stream) {
-  cudaError_t e = cudaFuncSetAttribute(attention_x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, X3_SMEM_BYTES);
-  if (e != cudaSuccess) return e;
-  const int grid = a.batch * a.heads * a.q_tiles;
-  attention_x3_kernel<<<grid, X3_THREADS, X3_SMEM_BYTES, stream>>>(tq3, tk3, tv2, a);
-  return cudaGetLastError();
+  return launch(attention_x3_kernel, a.batch * a.heads * a.q_tiles, X3_THREADS, X3_SMEM_BYTES, stream, false, tq3, tk3, tv2,
+                a);
 }
 
 // ---------------------------------------------------------------- operand preparation
@@ -228,10 +225,9 @@ cudaError_t launch_attn_split(const float* q, int ldq, const float* kv, int ldkv
   const size_t total = (rows_q + 2 * rows_kv) * heads * 16;
   if (total == 0) return cudaSuccess;
   const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
-  attn_split_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4*>(q), ldq / 4,
-                                              reinterpret_cast<const float4*>(kv), ldkv / 4, static_cast<uint2*>(q3),
-                                              static_cast<uint2*>(k3), static_cast<uint2*>(v2), rows_q, rows_kv, heads);
-  return cudaGetLastError();
+  return launch(attn_split_kernel, grid, 256, 0, stream, false, reinterpret_cast<const float4*>(q), ldq / 4,
+                reinterpret_cast<const float4*>(kv), ldkv / 4, static_cast<uint2*>(q3), static_cast<uint2*>(k3),
+                static_cast<uint2*>(v2), rows_q, rows_kv, heads);
 }
 
 // ---------------------------------------------------------------- GEMM operand split
@@ -256,8 +252,8 @@ cudaError_t launch_split3(const float* in, void* out, size_t rows, int k, int re
   const size_t total = rows * (k / 4);
   if (total == 0) return cudaSuccess;
   const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
-  split3_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4*>(in), static_cast<uint2*>(out), rows, k / 4, relu);
-  return cudaGetLastError();
+  return launch(split3_kernel, grid, 256, 0, stream, false, reinterpret_cast<const float4*>(in), static_cast<uint2*>(out),
+                rows, k / 4, relu);
 }
 
 // dst += src (fp32; second residual operand of the DPT fusion blocks in parity mode)
@@ -275,8 +271,8 @@ cudaError_t launch_add_f32(float* dst, const float* src, size_t n, cudaStream_t 
   if (n == 0) return cudaSuccess;
   const size_t n4 = n / 4;
   const int grid = static_cast<int>(n4 / 256 + 1 < 132 * 16 ? n4 / 256 + 1 : 132 * 16);
-  add_f32_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<float4*>(dst), reinterpret_cast<const float4*>(src), n4);
-  return cudaGetLastError();
+  return launch(add_f32_kernel, grid, 256, 0, stream, false, reinterpret_cast<float4*>(dst),
+                reinterpret_cast<const float4*>(src), n4);
 }
 
 }  // namespace f3r

@@ -1,7 +1,6 @@
 // extern "C" boundary of libfast3r_b200.so (see include/fast3r_b200.h).  Builds the TMA descriptors
 // (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint, so libcuda is not a link-time dependency),
 // validates arguments and enqueues the kernels on the caller's stream.
-#include <atomic>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -13,7 +12,6 @@
 namespace {
 
 thread_local char g_err[512] = "";
-std::atomic<uint64_t> g_launches{0};
 
 int fail(const char* fmt, ...) {
   va_list ap;
@@ -80,7 +78,7 @@ extern "C" {
 const char* f3r_last_error(void) { return g_err; }
 int f3r_abi_version(void) { return F3R_ABI_VERSION; }
 size_t f3r_gemm_desc_size(void) { return sizeof(f3r_gemm_desc); }
-uint64_t f3r_launch_count(void) { return g_launches.load(); }
+uint64_t f3r_launch_count(void) { return f3r::g_launch_count.load(); }
 
 int f3r_set_option(const char* name, int32_t value) {
   if (!name) return fail("f3r_set_option: null name");
@@ -205,7 +203,6 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
       if (cost < best - 1e-9) { best = cost; a.k_split = s; }
     }
   }
-  g_launches++;
   return check(f3r::launch_gemm(block_n, ta, tb, to0, to0b, a, num_sms(), static_cast<cudaStream_t>(stream)),
                "f3r_gemm");
 }
@@ -244,7 +241,6 @@ static int attention_impl(const char* what, const void* q, int32_t ldq, const vo
   a.scale_log2 = scale * 1.4426950408889634f;
   a.ldo = ldo; a.out = out; a.lse = lse;
   a.kv_row0 = kv_row0; a.n_split = n_split; a.part_base = part_base; a.part_o = part_o; a.part_lse = part_lse;
-  g_launches++;
   return check(f3r::launch_attention(tq, tkv, a, static_cast<cudaStream_t>(stream)), what);
 }
 
@@ -268,7 +264,6 @@ int f3r_attention_merge(const float* part_o, const float* part_lse, int32_t n_pa
                         int32_t batch, int32_t heads, int32_t sq, void* stream) {
   if (!part_o || !part_lse || !out || n_parts < 1) return fail("f3r_attention_merge: bad arguments");
   if (ldo % 8 || ldo < heads * 64) return fail("f3r_attention_merge: bad leading dimension");
-  g_launches++;
   return check(f3r::launch_attention_merge(part_o, part_lse, n_parts, batch, heads, sq, out, ldo,
                                            static_cast<cudaStream_t>(stream)), "f3r_attention_merge");
 }
@@ -276,14 +271,12 @@ int f3r_attention_merge(const float* part_o, const float* part_lse, int32_t n_pa
 int f3r_layernorm(const float* x, const float* w, const float* b, void* out, int32_t out_f32, int32_t rows,
                   int32_t dim, float eps, void* stream) {
   if (!x || !w || !b || !out) return fail("f3r_layernorm: null operand");
-  g_launches++;
   return check(f3r::launch_layernorm(x, w, b, out, out_f32, rows, dim, eps, static_cast<cudaStream_t>(stream)),
                "f3r_layernorm (dim must be one of 128,256,384,512,768,1024)");
 }
 
 int f3r_im2col_patch(const float* img, void* out, int32_t out_f32, int32_t n, int32_t h, int32_t w, void* stream) {
   if (!img || !out) return fail("f3r_im2col_patch: null operand");
-  g_launches++;
   return check(f3r::launch_im2col_patch(img, out, out_f32, n, h, w, 16, static_cast<cudaStream_t>(stream)),
                "f3r_im2col_patch");
 }
@@ -291,7 +284,6 @@ int f3r_im2col_patch(const float* img, void* out, int32_t out_f32, int32_t n, in
 int f3r_im2col3x3s2(const void* in, void* out, int32_t n, int32_t h, int32_t w, int32_t c, int32_t ho, int32_t wo,
                     void* stream) {
   if (!in || !out) return fail("f3r_im2col3x3s2: null operand");
-  g_launches++;
   return check(f3r::launch_im2col3x3s2(in, out, n, h, w, c, ho, wo, static_cast<cudaStream_t>(stream)),
                "f3r_im2col3x3s2");
 }
@@ -300,7 +292,6 @@ int f3r_upsample2x(const void* in, void* out, int32_t f32, int32_t n, int32_t h,
                    int32_t wo, void* stream) {
   if (!in || !out) return fail("f3r_upsample2x: null operand");
   if (ho > 2 * h || wo > 2 * w) return fail("f3r_upsample2x: window larger than the x2 output");
-  g_launches++;
   return check(f3r::launch_upsample2x(in, out, f32, n, h, w, c, ho, wo, 2 * h, 2 * w,
                                       static_cast<cudaStream_t>(stream)),
                "f3r_upsample2x");
@@ -309,13 +300,11 @@ int f3r_upsample2x(const void* in, void* out, int32_t f32, int32_t n, int32_t h,
 int f3r_split3(const float* in, void* out, size_t rows, int32_t k, int32_t relu, void* stream) {
   if (!in || !out) return fail("f3r_split3: null operand");
   if (k <= 0 || k % 8) return fail("f3r_split3: k=%d must be a positive multiple of 8", k);
-  g_launches++;
   return check(f3r::launch_split3(in, out, rows, k, relu, static_cast<cudaStream_t>(stream)), "f3r_split3");
 }
 
 int f3r_add_f32(float* dst, const float* src, size_t count, void* stream) {
   if (!dst || !src) return fail("f3r_add_f32: null operand");
-  g_launches++;
   return check(f3r::launch_add_f32(dst, src, count, static_cast<cudaStream_t>(stream)), "f3r_add_f32");
 }
 
@@ -343,7 +332,6 @@ int f3r_attention_x3(const float* q, int32_t ldq, const float* kv, int32_t ldkv,
   void* k3 = w + al(static_cast<size_t>(batch) * sq * heads * 192 * 2);
   void* v2 = static_cast<uint8_t*>(k3) + al(static_cast<size_t>(batch) * skv * heads * 192 * 2);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  g_launches++;
   if (check(f3r::launch_attn_split(q, ldq, kv, ldkv, q3, k3, v2, static_cast<size_t>(batch) * sq,
                                    static_cast<size_t>(batch) * skv, heads, st), "f3r_attention_x3 (split)"))
     return 1;
@@ -370,7 +358,6 @@ int f3r_attention_x3(const float* q, int32_t ldq, const float* kv, int32_t ldkv,
   a.q_tiles = (sq + 127) / 128;
   a.scale_log2 = scale * 1.4426950408889634f;
   a.ldo = ldo; a.out = out; a.lse = lse;
-  g_launches++;
   return check(f3r::launch_attention_x3(tq3, tk3, tv2, a, st), "f3r_attention_x3");
 }
 
@@ -397,7 +384,6 @@ int f3r_ingest_rgb8(const uint8_t* src, int32_t h, int32_t w, int32_t oh, int32_
     return fail("f3r_ingest_rgb8: tap tables must be given exactly for the resized dimensions");
   if (hk && (!hb || !tmp || hks <= 0 || h_span_max <= 0)) return fail("f3r_ingest_rgb8: incomplete horizontal pass arguments");
   if (vk && (!vb || vks <= 0)) return fail("f3r_ingest_rgb8: incomplete vertical pass arguments");
-  g_launches += hk ? 2 : 1;
   return check(f3r::launch_ingest(src, h, w, oh, ow, hb, hk, hks, h_span_max, vb, vk, vks, tmp, left, top, cw, ch, out,
                                   static_cast<cudaStream_t>(stream)), "f3r_ingest_rgb8");
 }
@@ -413,11 +399,8 @@ int f3r_jpeg_decode(const uint8_t* data, size_t size, const uint8_t* data_dev, i
                     int32_t left, int32_t top, int32_t out_w, int32_t out_h, uint8_t* out, int32_t* status_dev,
                     void* workspace, size_t workspace_bytes, void* stream) {
   if (!data || !data_dev || !out || !status_dev || !workspace) return fail("f3r_jpeg_decode: null operand");
-  int launches = 0;
   const char* err = f3r::launch_jpeg_decode(data, size, data_dev, orientation, rotate_cw90, left, top, out_w, out_h, out,
-                                            status_dev, workspace, workspace_bytes, static_cast<cudaStream_t>(stream),
-                                            &launches);
-  g_launches += launches;
+                                            status_dev, workspace, workspace_bytes, static_cast<cudaStream_t>(stream));
   return err ? fail("f3r_jpeg_decode: %s", err) : 0;
 }
 
@@ -426,7 +409,6 @@ int f3r_conf_quantile(const float* conf, int32_t views, int32_t n, float q, floa
   if (!conf || !thr) return fail("f3r_conf_quantile: null operand");
   if (views <= 0 || n <= 0 || n > (1 << 24)) return fail("f3r_conf_quantile: bad shape (n must be in [1, 2^24]: ranks are fp32)");
   if (!(q >= 0.f && q <= 1.f)) return fail("f3r_conf_quantile: q must be in [0, 1]");
-  g_launches++;
   return check(f3r::launch_conf_quantile(conf, views, n, q, thr, static_cast<cudaStream_t>(stream)), "f3r_conf_quantile");
 }
 
@@ -439,7 +421,6 @@ int f3r_similarity_fit(const float* x, const float* y, const float* conf, const 
   if ((conf != nullptr) != (thr != nullptr)) return fail("f3r_similarity_fit: conf and thr must be given together");
   if (workspace_bytes < f3r::similarity_fit_workspace(views)) return fail("f3r_similarity_fit: workspace too small");
   if (reinterpret_cast<uintptr_t>(workspace) & 7) return fail("f3r_similarity_fit: workspace not 8-byte aligned");
-  g_launches += conf ? 4 : 2;
   return check(f3r::launch_similarity_fit(x, y, conf, thr, valid, views, n, rts, static_cast<double*>(workspace),
                                           static_cast<cudaStream_t>(stream)), "f3r_similarity_fit");
 }
@@ -447,7 +428,6 @@ int f3r_similarity_fit(const float* x, const float* y, const float* conf, const 
 int f3r_similarity_apply(const float* x, const float* rts, float* out, int32_t views, int32_t n, void* stream) {
   if (!x || !rts || !out) return fail("f3r_similarity_apply: null operand");
   if (views <= 0 || views > 65535 || n <= 0 || n > (1 << 29)) return fail("f3r_similarity_apply: bad shape");
-  g_launches++;
   return check(f3r::launch_similarity_apply(x, rts, out, views, n, static_cast<cudaStream_t>(stream)), "f3r_similarity_apply");
 }
 
@@ -462,7 +442,6 @@ int f3r_focal_weiszfeld(const float* pts, const float* conf, const float* thr, c
   if ((conf != nullptr) != (thr != nullptr)) return fail("f3r_focal_weiszfeld: conf and thr must be given together");
   if (workspace_bytes < f3r::focal_workspace(views)) return fail("f3r_focal_weiszfeld: workspace too small");
   if (reinterpret_cast<uintptr_t>(workspace) & 7) return fail("f3r_focal_weiszfeld: workspace not 8-byte aligned");
-  g_launches += static_cast<uint64_t>(iters) + 2;
   return check(f3r::launch_focal_weiszfeld(pts, conf, thr, pp, views, h, w, iters, focal, static_cast<double*>(workspace),
                                            static_cast<cudaStream_t>(stream)), "f3r_focal_weiszfeld");
 }
@@ -475,10 +454,7 @@ int f3r_pc_index_build(const void* pts, int32_t f64, int32_t n, void* index, siz
   if (n <= 0) return fail("f3r_pc_index_build: bad size n=%d (must be >= 1)", n);
   if (index_bytes < f3r::pc_index_workspace(n)) return fail("f3r_pc_index_build: index block too small");
   if (reinterpret_cast<uintptr_t>(index) & 255) return fail("f3r_pc_index_build: index block not 256-byte aligned");
-  int launches = 0;
-  const cudaError_t e = f3r::launch_pc_index_build(pts, f64 != 0, n, index, static_cast<cudaStream_t>(stream), &launches);
-  g_launches += launches;
-  return check(e, "f3r_pc_index_build");
+  return check(f3r::launch_pc_index_build(pts, f64 != 0, n, index, static_cast<cudaStream_t>(stream)), "f3r_pc_index_build");
 }
 
 size_t f3r_pc_query_workspace(int32_t nq) { return nq > 0 ? f3r::pc_query_workspace(nq) : 0; }
@@ -494,11 +470,8 @@ int f3r_pc_nearest(const void* index, size_t index_bytes, int32_t n_ref, const v
     if ((reinterpret_cast<uintptr_t>(index) | reinterpret_cast<uintptr_t>(workspace)) & 255)
       return fail("f3r_pc_nearest: index or workspace not 256-byte aligned");
   }
-  int launches = 0;
-  const cudaError_t e = f3r::launch_pc_nearest(index, n_ref, query, f64 != 0, nq, dist, reinterpret_cast<long long*>(idx),
-                                               workspace, static_cast<cudaStream_t>(stream), &launches);
-  g_launches += launches;
-  return check(e, "f3r_pc_nearest");
+  return check(f3r::launch_pc_nearest(index, n_ref, query, f64 != 0, nq, dist, reinterpret_cast<long long*>(idx), workspace,
+                                       static_cast<cudaStream_t>(stream)), "f3r_pc_nearest");
 }
 
 int f3r_pc_knn_normals(const void* index, size_t index_bytes, int32_t n, int32_t k, double* normals, void* stream) {
@@ -507,14 +480,12 @@ int f3r_pc_knn_normals(const void* index, size_t index_bytes, int32_t n, int32_t
   if (k < 1 || k > 32) return fail("f3r_pc_knn_normals: k=%d must be in [1, 32]", k);
   if (index_bytes < f3r::pc_index_workspace(n)) return fail("f3r_pc_knn_normals: index block too small");
   if (reinterpret_cast<uintptr_t>(index) & 255) return fail("f3r_pc_knn_normals: index block not 256-byte aligned");
-  g_launches++;
   return check(f3r::launch_pc_knn_normals(index, n, k, normals, static_cast<cudaStream_t>(stream)), "f3r_pc_knn_normals");
 }
 
 int f3r_pc_count_nonfinite(const void* pts, int32_t f64, int32_t n, uint32_t* count, void* stream) {
   if (!count || (!pts && n)) return fail("f3r_pc_count_nonfinite: null operand");
   if (n < 0) return fail("f3r_pc_count_nonfinite: bad size n=%d", n);
-  g_launches++;
   return check(f3r::launch_pc_count_nonfinite(pts, f64 != 0, n, count, static_cast<cudaStream_t>(stream)),
                "f3r_pc_count_nonfinite");
 }
@@ -523,7 +494,6 @@ int f3r_pc_abs_dot(const double* a, const int64_t* a_idx, const double* b, const
                    void* stream) {
   if (!a || !b || !out) return fail("f3r_pc_abs_dot: null operand");
   if (n < 0) return fail("f3r_pc_abs_dot: bad size n=%d", n);
-  g_launches++;
   return check(f3r::launch_pc_abs_dot(a, reinterpret_cast<const long long*>(a_idx), b,
                                       reinterpret_cast<const long long*>(b_idx), n, out, static_cast<cudaStream_t>(stream)),
                "f3r_pc_abs_dot");
@@ -542,29 +512,23 @@ static int reduce_args(const char* what, const double* x, int32_t n, const doubl
 
 int f3r_f64_mean(const double* x, int32_t n, double* out, void* workspace, size_t workspace_bytes, void* stream) {
   if (reduce_args("f3r_f64_mean", x, n, out, workspace, workspace_bytes)) return 1;
-  g_launches += 2;
   return check(f3r::launch_f64_mean(x, n, out, workspace, static_cast<cudaStream_t>(stream)), "f3r_f64_mean");
 }
 
 int f3r_f64_median(const double* x, int32_t n, double* out, void* workspace, size_t workspace_bytes, void* stream) {
   if (reduce_args("f3r_f64_median", x, n, out, workspace, workspace_bytes)) return 1;
-  int launches = 0;
-  const cudaError_t e = f3r::launch_f64_median(x, n, out, workspace, static_cast<cudaStream_t>(stream), &launches);
-  g_launches += launches;
-  return check(e, "f3r_f64_median");
+  return check(f3r::launch_f64_median(x, n, out, workspace, static_cast<cudaStream_t>(stream)), "f3r_f64_median");
 }
 
 int f3r_f64_count_below(const double* x, int32_t n, const double* th, uint64_t* count, void* stream) {
   if (!th || !count || (!x && n)) return fail("f3r_f64_count_below: null operand");
   if (n < 0) return fail("f3r_f64_count_below: bad size n=%d", n);
-  g_launches++;
   return check(f3r::launch_f64_count_below(x, n, th, reinterpret_cast<unsigned long long*>(count),
                                            static_cast<cudaStream_t>(stream)), "f3r_f64_count_below");
 }
 
 int f3r_cast_bf16(const float* in, void* out, size_t count, void* stream) {
   if (!in || !out) return fail("f3r_cast_bf16: null operand");
-  g_launches++;
   return check(f3r::launch_cast_bf16(in, out, count, static_cast<cudaStream_t>(stream)), "f3r_cast_bf16");
 }
 

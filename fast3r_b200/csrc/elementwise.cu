@@ -15,22 +15,7 @@ bool pdl_enabled() {
   }
   return g_pdl == 1;
 }
-int launch_attrs(cudaLaunchAttribute* attr, int cluster) {
-  int n = 0;
-  if (cluster > 1) {
-    attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = cluster;
-    attr[n].val.clusterDim.y = 1;
-    attr[n].val.clusterDim.z = 1;
-    ++n;
-  }
-  if (pdl_enabled()) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  return n;
-}
+std::atomic<uint64_t> g_launch_count{0};
 
 // ---------------------------------------------------------------- LayerNorm
 // nn.LayerNorm over the last dim, biased variance, y = (x-mu)/sqrt(var+eps)*w+b.  One warp per row.
@@ -87,23 +72,17 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 cudaError_t launch_layernorm(const float* x, const float* w, const float* b, void* out, int out_f32, int rows,
                              int dim, float eps, cudaStream_t stream) {
   if (rows <= 0) return cudaSuccess;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((rows + 7) / 8);
-  cfg.blockDim = dim3(256);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  cfg.attrs = attr;
-  cfg.numAttrs = launch_attrs(attr, 1);
+  decltype(&layernorm_kernel<1>) kernel;
   switch (dim) {
-    case 128: return cudaLaunchKernelEx(&cfg, layernorm_kernel<1>, x, w, b, out, out_f32, rows, eps);
-    case 256: return cudaLaunchKernelEx(&cfg, layernorm_kernel<2>, x, w, b, out, out_f32, rows, eps);
-    case 384: return cudaLaunchKernelEx(&cfg, layernorm_kernel<3>, x, w, b, out, out_f32, rows, eps);
-    case 512: return cudaLaunchKernelEx(&cfg, layernorm_kernel<4>, x, w, b, out, out_f32, rows, eps);
-    case 768: return cudaLaunchKernelEx(&cfg, layernorm_kernel<6>, x, w, b, out, out_f32, rows, eps);
-    case 1024: return cudaLaunchKernelEx(&cfg, layernorm_kernel<8>, x, w, b, out, out_f32, rows, eps);
+    case 128: kernel = layernorm_kernel<1>; break;
+    case 256: kernel = layernorm_kernel<2>; break;
+    case 384: kernel = layernorm_kernel<3>; break;
+    case 512: kernel = layernorm_kernel<4>; break;
+    case 768: kernel = layernorm_kernel<6>; break;
+    case 1024: kernel = layernorm_kernel<8>; break;
     default: return cudaErrorInvalidValue;
   }
-  return cudaGetLastError();
+  return launch(kernel, (rows + 7) / 8, 256, 0, stream, true, x, w, b, out, out_f32, rows, eps);
 }
 
 // ---------------------------------------------------------------- patch im2col
@@ -141,9 +120,8 @@ cudaError_t launch_im2col_patch(const float* img, void* out, int out_f32, int n,
   const size_t total = static_cast<size_t>(n) * (H / 16) * (W / 16) * 96;
   if (total == 0) return cudaSuccess;
   const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
-  if (out_f32) im2col_patch_kernel<true><<<grid, 256, 0, stream>>>(img, out, n, H, W);
-  else im2col_patch_kernel<false><<<grid, 256, 0, stream>>>(img, out, n, H, W);
-  return cudaGetLastError();
+  return launch(out_f32 ? im2col_patch_kernel<true> : im2col_patch_kernel<false>, grid, 256, 0, stream, false, img, out, n,
+                H, W);
 }
 
 // ---------------------------------------------------------------- 3x3 stride-2 pad-1 im2col (NHWC bf16)
@@ -170,9 +148,8 @@ cudaError_t launch_im2col3x3s2(const void* in, void* out, int n, int H, int W, i
   const size_t total = static_cast<size_t>(n) * Ho * Wo * 9 * (C / 8);
   if (total == 0) return cudaSuccess;
   const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
-  im2col3x3s2_kernel<<<grid, 256, 0, stream>>>(static_cast<const uint4*>(in), static_cast<uint4*>(out), n, H, W,
-                                               C / 8, Ho, Wo);
-  return cudaGetLastError();
+  return launch(im2col3x3s2_kernel, grid, 256, 0, stream, false, static_cast<const uint4*>(in), static_cast<uint4*>(out), n,
+                H, W, C / 8, Ho, Wo);
 }
 
 // ---------------------------------------------------------------- bilinear x2, align_corners=True (NHWC bf16)
@@ -258,9 +235,8 @@ cudaError_t launch_upsample2x(const void* in, void* out, int f32, int n, int H, 
     const float sy = static_cast<float>(H - 1) / static_cast<float>(Hfull - 1);
     const float sx = static_cast<float>(W - 1) / static_cast<float>(Wfull - 1);
     dim3 grid((Wo * C4 + 255) / 256, Ho, n);
-    upsample2x_f32_kernel<<<grid, 256, 0, stream>>>(static_cast<const float4*>(in), static_cast<float4*>(out), H, W, C4,
-                                                    shift, Ho, Wo, sy, sx);
-    return cudaGetLastError();
+    return launch(upsample2x_f32_kernel, grid, 256, 0, stream, false, static_cast<const float4*>(in),
+                  static_cast<float4*>(out), H, W, C4, shift, Ho, Wo, sy, sx);
   }
   const int C8 = C / 8;
   int shift = 0;
@@ -271,9 +247,8 @@ cudaError_t launch_upsample2x(const void* in, void* out, int f32, int n, int H, 
   const float sy = static_cast<float>(H - 1) / static_cast<float>(Hfull - 1);
   const float sx = static_cast<float>(W - 1) / static_cast<float>(Wfull - 1);
   dim3 grid((Wo * C8 + 255) / 256, (Ho + UPS_ROWS - 1) / UPS_ROWS, n);
-  upsample2x_kernel<<<grid, 256, 0, stream>>>(static_cast<const uint4*>(in), static_cast<uint4*>(out), H, W, C8, shift,
-                                              Ho, Wo, sy, sx);
-  return cudaGetLastError();
+  return launch(upsample2x_kernel, grid, 256, 0, stream, false, static_cast<const uint4*>(in), static_cast<uint4*>(out), H,
+                W, C8, shift, Ho, Wo, sy, sx);
 }
 
 // ---------------------------------------------------------------- fp32 -> bf16
@@ -290,8 +265,8 @@ cudaError_t launch_cast_bf16(const float* in, void* out, size_t n, cudaStream_t 
   if (n == 0) return cudaSuccess;
   const size_t n4 = n / 4;
   const int grid = static_cast<int>(n4 / 256 + 1 < 132 * 16 ? n4 / 256 + 1 : 132 * 16);
-  cast_bf16_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const float4*>(in), static_cast<uint2*>(out), n4);
-  return cudaGetLastError();
+  return launch(cast_bf16_kernel, grid, 256, 0, stream, false, reinterpret_cast<const float4*>(in),
+                static_cast<uint2*>(out), n4);
 }
 
 }  // namespace f3r

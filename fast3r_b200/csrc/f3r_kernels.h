@@ -4,6 +4,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+#include <utility>
+
 #include "../../include/fast3r_b200.h"
 
 namespace f3r {
@@ -11,8 +14,47 @@ namespace f3r {
 // 1: launch the hot-chain kernels with programmatic stream serialization (PDL); F3R_PDL=0 / f3r_set_option("pdl", 0) disable
 extern int g_pdl;
 bool pdl_enabled();
-// fills `attr` (room for 2) with the cluster dimension (if cluster > 1) and the PDL attribute (if enabled); returns the count
-int launch_attrs(cudaLaunchAttribute* attr, int cluster);
+// kernels launched by launch() so far (f3r_launch_count)
+extern std::atomic<uint64_t> g_launch_count;
+
+// Every kernel of the library is launched here, so g_launch_count counts exactly the launches that were enqueued.
+// pdl: programmatic stream serialization (if pdl_enabled()), for the kernels that execute griddepcontrol.
+// kCluster > 1: thread-block clusters of kCluster CTAs along x.  Dynamic shared memory above 48 KB is opted into on
+// every launch: the attribute is per device and one process may drive several GPUs.
+template <int kCluster = 1, typename... Params, typename... Args>
+cudaError_t launch(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl,
+                   Args&&... args) {
+  if (smem > 48 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    if (e != cudaSuccess) return e;
+  }
+  cudaLaunchAttribute attr[2];
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  if (kCluster > 1) {
+    attr[cfg.numAttrs].id = cudaLaunchAttributeClusterDimension;
+    attr[cfg.numAttrs].val.clusterDim.x = kCluster;
+    attr[cfg.numAttrs].val.clusterDim.y = 1;
+    attr[cfg.numAttrs].val.clusterDim.z = 1;
+    ++cfg.numAttrs;
+  }
+  if (pdl && pdl_enabled()) {
+    attr[cfg.numAttrs].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[cfg.numAttrs].val.programmaticStreamSerializationAllowed = 1;
+    ++cfg.numAttrs;
+  }
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // the error is returned here; do not leave it behind for the caller's next CUDA error check
+    return e;
+  }
+  ++g_launch_count;
+  return e;
+}
 
 enum { EPI_STORE = 0, EPI_ROPE = 1, EPI_IDXEMB = 2, EPI_CONVT = 3, EPI_FINAL = 4 };
 enum { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2 };
@@ -95,7 +137,7 @@ cudaError_t launch_cast_bf16(const float* in, void* out, size_t n, cudaStream_t 
 const char* jpeg_probe(const uint8_t* data, size_t size, f3r_jpeg_info* info);
 const char* launch_jpeg_decode(const uint8_t* data, size_t size, const uint8_t* data_dev, int orientation, int rotate_cw90,
                                int left, int top, int out_w, int out_h, uint8_t* out, int32_t* status, void* workspace,
-                               size_t workspace_bytes, cudaStream_t stream, int* launches);
+                               size_t workspace_bytes, cudaStream_t stream);
 
 // image ingest (ingest.cu)
 int resample_ksize(int in_size, int out_size, int filter);
@@ -119,15 +161,15 @@ cudaError_t launch_focal_weiszfeld(const float* pts, const float* conf, const fl
 size_t pc_index_workspace(int n);
 size_t pc_query_workspace(int nq);
 size_t f64_reduce_workspace();
-cudaError_t launch_pc_index_build(const void* pts, int f64, int n, void* index, cudaStream_t stream, int* launches);
+cudaError_t launch_pc_index_build(const void* pts, int f64, int n, void* index, cudaStream_t stream);
 cudaError_t launch_pc_nearest(const void* index, int n_ref, const void* query, int f64, int nq, double* dist,
-                              long long* idx, void* workspace, cudaStream_t stream, int* launches);
+                              long long* idx, void* workspace, cudaStream_t stream);
 cudaError_t launch_pc_knn_normals(const void* index, int n, int k, double* normals, cudaStream_t stream);
 cudaError_t launch_pc_count_nonfinite(const void* pts, int f64, int n, unsigned int* count, cudaStream_t stream);
 cudaError_t launch_pc_abs_dot(const double* a, const long long* a_idx, const double* b, const long long* b_idx, int n,
                               double* out, cudaStream_t stream);
 cudaError_t launch_f64_mean(const double* x, int n, double* out, void* workspace, cudaStream_t stream);
-cudaError_t launch_f64_median(const double* x, int n, double* out, void* workspace, cudaStream_t stream, int* launches);
+cudaError_t launch_f64_median(const double* x, int n, double* out, void* workspace, cudaStream_t stream);
 cudaError_t launch_f64_count_below(const double* x, int n, const double* th, unsigned long long* count,
                                    cudaStream_t stream);
 

@@ -437,22 +437,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 template <int BLOCK_N>
 static cudaError_t launch_gemm_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
                                  const CUtensorMap& to0b, const GemmArgs& a, int num_sms, cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N>;
-  {  // (per launch: the attribute is per device and one process may drive several GPUs)
-    cudaError_t e = cudaFuncSetAttribute(gemm_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::kSmemBytes);
-    if (e != cudaSuccess) return e;
-  }
   const int items = a.num_m_tiles * a.num_n_tiles * a.k_split;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(items < num_sms ? items : num_sms);
-  cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  cfg.attrs = attr;
-  cfg.numAttrs = launch_attrs(attr, 1);
-  return cudaLaunchKernelEx(&cfg, gemm_kernel<BLOCK_N>, ta, tb, to0, to0b, a);
+  return launch(gemm_kernel<BLOCK_N>, items < num_sms ? items : num_sms, GEMM_THREADS, GemmCfg<BLOCK_N>::kSmemBytes,
+                stream, true, ta, tb, to0, to0b, a);
 }
 
 cudaError_t launch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,

@@ -448,18 +448,7 @@ __global__ void weiszfeld_final_kernel(const double* __restrict__ last, int view
 // ------------------------------------------------------------------------------------------------- launchers
 cudaError_t launch_conf_quantile(const float* conf, int views, int n, float q, float* thr, cudaStream_t stream) {
   const int vec_ok = (n % 4 == 0) && (reinterpret_cast<uintptr_t>(conf) & 15) == 0;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(static_cast<unsigned>(views) * QC);
-  cfg.blockDim = dim3(QT);
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = QC;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, conf_quantile_kernel, conf, n, q, thr, vec_ok);
+  return launch<QC>(conf_quantile_kernel, static_cast<unsigned>(views) * QC, QT, 0, stream, false, conf, n, q, thr, vec_ok);
 }
 
 // partial sums [views][FIT_CHUNKS][MOM] fp64, then one int flag per view
@@ -476,28 +465,21 @@ cudaError_t launch_similarity_fit(const float* x, const float* y, const float* c
   const int vec_ok = (n % 4 == 0) && (al & 15) == 0 && (reinterpret_cast<uintptr_t>(valid) & 3) == 0;
   const int modes = (conf && thr) ? 2 : 1;  // without a confidence mask the first fallback is the same point set
   for (int mode = 0; mode < modes; ++mode) {
-    similarity_moments_kernel<<<dim3(FIT_CHUNKS, views), FIT_THREADS, 0, stream>>>(x, y, conf, thr, valid, n, vec_ok, mode,
-                                                                                     flags, workspace);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
-    similarity_solve_kernel<<<views, 64, 0, stream>>>(workspace, rts, mode, flags);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
+    cudaError_t e;
+    if ((e = launch(similarity_moments_kernel, dim3(FIT_CHUNKS, views), FIT_THREADS, 0, stream, false, x, y, conf, thr,
+                    valid, n, vec_ok, mode, flags, workspace)) != cudaSuccess)
+      return e;
+    if ((e = launch(similarity_solve_kernel, views, 64, 0, stream, false, workspace, rts, mode, flags)) != cudaSuccess)
+      return e;
   }
   return cudaSuccess;
 }
 
 cudaError_t launch_similarity_apply(const float* x, const float* rts, float* out, int views, int n, cudaStream_t stream) {
   const bool vec = (n % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
-  if (vec) {
-    const int groups = n / 4;
-    similarity_apply_kernel<true><<<dim3((groups + APPLY_THREADS - 1) / APPLY_THREADS, views), APPLY_THREADS, 0, stream>>>(
-        x, rts, out, n);
-  } else {
-    similarity_apply_kernel<false><<<dim3((n + APPLY_THREADS - 1) / APPLY_THREADS, views), APPLY_THREADS, 0, stream>>>(
-        x, rts, out, n);
-  }
-  return cudaGetLastError();
+  const int items = vec ? n / 4 : n;
+  return launch(vec ? similarity_apply_kernel<true> : similarity_apply_kernel<false>,
+                dim3((items + APPLY_THREADS - 1) / APPLY_THREADS, views), APPLY_THREADS, 0, stream, false, x, rts, out, n);
 }
 
 size_t focal_workspace(int views) { return 2 * static_cast<size_t>(views) * FOC_CHUNKS * FOC_P * sizeof(double); }
@@ -508,13 +490,11 @@ cudaError_t launch_focal_weiszfeld(const float* pts, const float* conf, const fl
   double* buf[2] = {workspace, workspace + half};
   const dim3 grid(FOC_CHUNKS, views);
   for (int it = 0; it <= iters; ++it) {
-    weiszfeld_iter_kernel<<<grid, FOC_THREADS, 0, stream>>>(pts, conf, thr, pp, H, W, it ? buf[(it - 1) & 1] : nullptr,
-                                                            buf[it & 1]);
-    cudaError_t e = cudaGetLastError();
+    const cudaError_t e = launch(weiszfeld_iter_kernel, grid, FOC_THREADS, 0, stream, false, pts, conf, thr, pp, H, W,
+                                 it ? buf[(it - 1) & 1] : nullptr, buf[it & 1]);
     if (e != cudaSuccess) return e;
   }
-  weiszfeld_final_kernel<<<(views + 127) / 128, 128, 0, stream>>>(buf[iters & 1], views, H, W, focal);
-  return cudaGetLastError();
+  return launch(weiszfeld_final_kernel, (views + 127) / 128, 128, 0, stream, false, buf[iters & 1], views, H, W, focal);
 }
 
 }  // namespace f3r

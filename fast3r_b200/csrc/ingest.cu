@@ -127,18 +127,15 @@ cudaError_t launch_ingest(const uint8_t* src, int h, int w, int oh, int ow, cons
   if (hk != nullptr) {
     const size_t smem = static_cast<size_t>(hks) * ING_COLS * 4 + static_cast<size_t>(ING_ROWS) * (((h_span_max * 3 + 3) & ~3) + 4);
     if (smem > 200 * 1024) return cudaErrorInvalidValue;
-    cudaError_t e = cudaFuncSetAttribute(resize_h_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-    if (e != cudaSuccess) return e;
     dim3 grid((ow + ING_COLS - 1) / ING_COLS, (h + ING_ROWS_PER_BLOCK - 1) / ING_ROWS_PER_BLOCK);
-    resize_h_kernel<<<grid, ING_COLS * ING_ROWS, smem, stream>>>(src, h, w, tmp, ow, hb, hk, hks, h_span_max);
-    e = cudaGetLastError();
+    const cudaError_t e = launch(resize_h_kernel, grid, ING_COLS * ING_ROWS, smem, stream, false, src, h, w, tmp, ow, hb, hk,
+                                 hks, h_span_max);
     if (e != cudaSuccess) return e;
     mid = tmp;
   }
   dim3 grid((cw + 255) / 256, ch);
-  resize_v_crop_norm_kernel<<<grid, 256, 0, stream>>>(mid, ow, vb, vk, vks, left, top, cw, ch, out);
   (void)oh;
-  return cudaGetLastError();
+  return launch(resize_v_crop_norm_kernel, grid, 256, 0, stream, false, mid, ow, vb, vk, vks, left, top, cw, ch, out);
 }
 
 // ---------------------------------------------------------------- host: Pillow's coefficient tables

@@ -545,7 +545,7 @@ const char* jpeg_probe(const uint8_t* data, size_t size, f3r_jpeg_info* info) {
 
 const char* launch_jpeg_decode(const uint8_t* data, size_t size, const uint8_t* data_dev, int orientation, int rotate_cw90,
                                int left, int top, int out_w, int out_h, uint8_t* out, int32_t* status, void* workspace,
-                               size_t workspace_bytes, cudaStream_t stream, int* launches) {
+                               size_t workspace_bytes, cudaStream_t stream) {
   HeaderBox* b = new (std::nothrow) HeaderBox;
   if (!b) return "out of host memory";
   struct Free { HeaderBox* b; ~Free() { delete b; } } guard{b};
@@ -599,27 +599,26 @@ const char* launch_jpeg_decode(const uint8_t* data, size_t size, const uint8_t* 
   if ((e = cudaMemsetAsync(P.hdr, 0, (3 + MAX_ROUNDS) * 4, stream)) != cudaSuccess) return cudaGetErrorString(e);
   if ((e = cudaMemsetAsync(P.coef, 0, static_cast<size_t>(L.total_blocks) * 128, stream)) != cudaSuccess)
     return cudaGetErrorString(e);
-  int n = 0;
   const uint32_t nchunks = L.nchunks > 0 ? L.nchunks : 1;
-  jpeg_unstuff_count_kernel<<<nchunks, UNSTUFF_THREADS, 0, stream>>>(P);
-  jpeg_chunk_scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(P, L.nchunks);
-  jpeg_unstuff_write_kernel<<<nchunks, UNSTUFF_THREADS, 0, stream>>>(P);
-  n += 3;
   const uint32_t sync_ctas = (L.nsub_max + SYNC_THREADS - 1) / SYNC_THREADS > 0 ? (L.nsub_max + SYNC_THREADS - 1) / SYNC_THREADS : 1;
-  jpeg_sync_init_kernel<<<(L.nsub_max + 2 + 255) / 256, 256, 0, stream>>>(P);
-  ++n;
-  for (int r = 0; r < MAX_ROUNDS; ++r, ++n) jpeg_sync_kernel<<<sync_ctas, SYNC_THREADS, 0, stream>>>(P, r);
-  jpeg_rec_scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(P);
-  jpeg_write_kernel<<<sync_ctas, SYNC_THREADS, 0, stream>>>(P);
-  jpeg_idct_kernel<<<(L.total_blocks + 127) / 128, 128, 0, stream>>>(P);
   Map M;
   jpeg::orient_map(h.width, h.height, orientation, rotate_cw90, left, top, M.m);
-  jpeg_color_kernel<<<dim3((out_w + 255) / 256, out_h), 256, 0, stream>>>(P, M, out_w, out_h, out);
-  jpeg_finish_kernel<<<1, 1, 0, stream>>>(P, status);
-  n += 5;
-  *launches = n;
-  e = cudaGetLastError();
-  return e == cudaSuccess ? nullptr : cudaGetErrorString(e);
+  if ((e = launch(jpeg_unstuff_count_kernel, nchunks, UNSTUFF_THREADS, 0, stream, false, P)) != cudaSuccess ||
+      (e = launch(jpeg_chunk_scan_kernel, 1, SCAN_THREADS, 0, stream, false, P, L.nchunks)) != cudaSuccess ||
+      (e = launch(jpeg_unstuff_write_kernel, nchunks, UNSTUFF_THREADS, 0, stream, false, P)) != cudaSuccess ||
+      (e = launch(jpeg_sync_init_kernel, (L.nsub_max + 2 + 255) / 256, 256, 0, stream, false, P)) != cudaSuccess)
+    return cudaGetErrorString(e);
+  for (int r = 0; r < MAX_ROUNDS; ++r)
+    if ((e = launch(jpeg_sync_kernel, sync_ctas, SYNC_THREADS, 0, stream, false, P, r)) != cudaSuccess)
+      return cudaGetErrorString(e);
+  if ((e = launch(jpeg_rec_scan_kernel, 1, SCAN_THREADS, 0, stream, false, P)) != cudaSuccess ||
+      (e = launch(jpeg_write_kernel, sync_ctas, SYNC_THREADS, 0, stream, false, P)) != cudaSuccess ||
+      (e = launch(jpeg_idct_kernel, (L.total_blocks + 127) / 128, 128, 0, stream, false, P)) != cudaSuccess ||
+      (e = launch(jpeg_color_kernel, dim3((out_w + 255) / 256, out_h), 256, 0, stream, false, P, M, out_w, out_h,
+                  out)) != cudaSuccess ||
+      (e = launch(jpeg_finish_kernel, 1, 1, 0, stream, false, P, status)) != cudaSuccess)
+    return cudaGetErrorString(e);
+  return nullptr;
 }
 
 }  // namespace f3r

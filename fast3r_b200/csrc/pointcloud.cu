@@ -311,11 +311,12 @@ cudaError_t radix_sort(unsigned long long* k[2], int* v[2], int n, int bits, uin
   const int tiles = sort_tiles(n);
   for (int shift = 0; shift < bits; shift += 8) {
     const int a = *in_b, b = 1 - a;
-    sort_hist_kernel<<<tiles, ST, 0, st>>>(k[a], n, shift, hist, tiles);
-    sort_scan_kernel<<<1, SCAN_T, 0, st>>>(hist, tiles * 256);
-    sort_scatter_kernel<<<tiles, ST, 0, st>>>(k[a], v[a], k[b], v[b], n, shift, hist, tiles);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
+    cudaError_t e;
+    if ((e = launch(sort_hist_kernel, tiles, ST, 0, st, false, k[a], n, shift, hist, tiles)) != cudaSuccess) return e;
+    if ((e = launch(sort_scan_kernel, 1, SCAN_T, 0, st, false, hist, tiles * 256)) != cudaSuccess) return e;
+    if ((e = launch(sort_scatter_kernel, tiles, ST, 0, st, false, k[a], v[a], k[b], v[b], n, shift, hist, tiles)) !=
+        cudaSuccess)
+      return e;
     *in_b = b;
   }
   return cudaSuccess;
@@ -705,7 +706,7 @@ size_t pc_index_workspace(int n) { return index_layout(n).total; }
 size_t pc_query_workspace(int nq) { return query_layout(nq).total; }
 size_t f64_reduce_workspace() { return al256(sizeof(SelState)) + al256(256 * 4) + al256(RED_BLOCKS * 8); }
 
-cudaError_t launch_pc_index_build(const void* pts, int f64, int n, void* index, cudaStream_t st, int* launches) {
+cudaError_t launch_pc_index_build(const void* pts, int f64, int n, void* index, cudaStream_t st) {
   const IndexLayout l = index_layout(n);
   uint8_t* b = static_cast<uint8_t*>(index);
   Header* h = reinterpret_cast<Header*>(b + l.hdr);
@@ -715,37 +716,34 @@ cudaError_t launch_pc_index_build(const void* pts, int f64, int n, void* index, 
   unsigned long long* hi = reinterpret_cast<unsigned long long*>(b + l.lo);
   uint32_t* hist = reinterpret_cast<uint32_t*>(b + l.hist);
   const int g = (n + 255) / 256;
-  pc_bbox_init_kernel<<<1, 32, 0, st>>>(h);
-  pc_bbox_kernel<<<min(g, 1024), 256, 0, st>>>(pts, f64, n, h);
-  pc_bbox_finish_kernel<<<1, 32, 0, st>>>(h);
-  pc_code_kernel<<<g, 256, 0, st>>>(pts, f64, n, h, k[0], v[0], hi, 0);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
+  cudaError_t e;
+  if ((e = launch(pc_bbox_init_kernel, 1, 32, 0, st, false, h)) != cudaSuccess) return e;
+  if ((e = launch(pc_bbox_kernel, min(g, 1024), 256, 0, st, false, pts, f64, n, h)) != cudaSuccess) return e;
+  if ((e = launch(pc_bbox_finish_kernel, 1, 32, 0, st, false, h)) != cudaSuccess) return e;
+  if ((e = launch(pc_code_kernel, g, 256, 0, st, false, pts, f64, n, h, k[0], v[0], hi, 0)) != cudaSuccess) return e;
   int in_b = 0;
   if ((e = radix_sort(k, v, n, 36, hist, &in_b, st)) != cudaSuccess) return e;  // low 12 bits per axis (5 passes)
-  pc_gather_keys_kernel<<<g, 256, 0, st>>>(hi, v[in_b], k[1 - in_b], v[1 - in_b], n);
+  if ((e = launch(pc_gather_keys_kernel, g, 256, 0, st, false, hi, v[in_b], k[1 - in_b], v[1 - in_b], n)) != cudaSuccess)
+    return e;
   in_b = 1 - in_b;
   if ((e = radix_sort(k, v, n, 63, hist, &in_b, st)) != cudaSuccess) return e;  // 63-bit code (8 passes)
   // 13 passes in all: the sorted keys and permutation end where the index keeps them (buffer 0)
   double* pts_s = reinterpret_cast<double*>(b + l.pts);
-  pc_gather_points_kernel<<<g, 256, 0, st>>>(pts, f64, v[0], pts_s, n);
+  if ((e = launch(pc_gather_points_kernel, g, 256, 0, st, false, pts, f64, v[0], pts_s, n)) != cudaSuccess) return e;
   const Tree t = make_tree(n);
   double* nodes = reinterpret_cast<double*>(b + l.nodes);
-  pc_leaf_box_kernel<<<(t.cnt[0] + 127) / 128, 128, 0, st>>>(pts_s, n, nodes, t.cnt[0]);
+  if ((e = launch(pc_leaf_box_kernel, (t.cnt[0] + 127) / 128, 128, 0, st, false, pts_s, n, nodes, t.cnt[0])) != cudaSuccess)
+    return e;
   for (int lv = 1; lv < t.levels; ++lv)
-    pc_parent_box_kernel<<<(t.cnt[lv] + 127) / 128, 128, 0, st>>>(nodes + 6 * t.off[lv - 1], t.cnt[lv - 1],
-                                                                   nodes + 6 * t.off[lv], t.cnt[lv]);
-  *launches = 7 + 13 * 3 + t.levels;
-  return cudaGetLastError();
+    if ((e = launch(pc_parent_box_kernel, (t.cnt[lv] + 127) / 128, 128, 0, st, false, nodes + 6 * t.off[lv - 1],
+                    t.cnt[lv - 1], nodes + 6 * t.off[lv], t.cnt[lv])) != cudaSuccess)
+      return e;
+  return cudaSuccess;
 }
 
 cudaError_t launch_pc_nearest(const void* index, int n_ref, const void* query, int f64, int nq, double* dist,
-                              long long* idx, void* workspace, cudaStream_t st, int* launches) {
-  if (n_ref == 0) {
-    pc_fill_empty_kernel<<<(nq + 255) / 256, 256, 0, st>>>(nq, n_ref, dist, idx);
-    *launches = 1;
-    return cudaGetLastError();
-  }
+                              long long* idx, void* workspace, cudaStream_t st) {
+  if (n_ref == 0) return launch(pc_fill_empty_kernel, (nq + 255) / 256, 256, 0, st, false, nq, n_ref, dist, idx);
   const IndexView ix = index_view(index, n_ref);
   const QueryLayout l = query_layout(nq);
   uint8_t* w = static_cast<uint8_t*>(workspace);
@@ -753,21 +751,19 @@ cudaError_t launch_pc_nearest(const void* index, int n_ref, const void* query, i
                               reinterpret_cast<unsigned long long*>(w + l.keys_b)};
   int* v[2] = {reinterpret_cast<int*>(w + l.vals_a), reinterpret_cast<int*>(w + l.vals_b)};
   uint32_t* hist = reinterpret_cast<uint32_t*>(w + l.hist);
-  pc_code_kernel<<<(nq + 255) / 256, 256, 0, st>>>(query, f64, nq, ix.hdr, k[0], v[0], nullptr, 1);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return e;
+  cudaError_t e;
+  if ((e = launch(pc_code_kernel, (nq + 255) / 256, 256, 0, st, false, query, f64, nq, ix.hdr, k[0], v[0], nullptr, 1)) !=
+      cudaSuccess)
+    return e;
   int in_b = 0;
   if ((e = radix_sort(k, v, nq, 63, hist, &in_b, st)) != cudaSuccess) return e;
-  pc_nearest_kernel<<<(nq + PC_THREADS - 1) / PC_THREADS, PC_THREADS, 0, st>>>(ix, query, f64, nq, k[in_b], v[in_b], dist,
-                                                                               idx);
-  *launches = 2 + 8 * 3;
-  return cudaGetLastError();
+  return launch(pc_nearest_kernel, (nq + PC_THREADS - 1) / PC_THREADS, PC_THREADS, 0, st, false, ix, query, f64, nq,
+                k[in_b], v[in_b], dist, idx);
 }
 
 cudaError_t launch_pc_knn_normals(const void* index, int n, int k, double* normals, cudaStream_t st) {
   const IndexView ix = index_view(index, n);
-  pc_knn_normals_kernel<<<(n + PC_THREADS - 1) / PC_THREADS, PC_THREADS, 0, st>>>(ix, k, normals);
-  return cudaGetLastError();
+  return launch(pc_knn_normals_kernel, (n + PC_THREADS - 1) / PC_THREADS, PC_THREADS, 0, st, false, ix, k, normals);
 }
 
 cudaError_t launch_pc_count_nonfinite(const void* pts, int f64, int n, unsigned int* count, cudaStream_t st) {
@@ -775,45 +771,42 @@ cudaError_t launch_pc_count_nonfinite(const void* pts, int f64, int n, unsigned 
   if (e != cudaSuccess) return e;
   const long long c = 3ll * n;
   if (c == 0) return cudaSuccess;
-  pc_count_nonfinite_kernel<<<static_cast<int>(min(1024ll, (c + 255) / 256)), 256, 0, st>>>(pts, f64, c, count);
-  return cudaGetLastError();
+  return launch(pc_count_nonfinite_kernel, static_cast<int>(min(1024ll, (c + 255) / 256)), 256, 0, st, false, pts, f64, c,
+                count);
 }
 
 cudaError_t launch_pc_abs_dot(const double* a, const long long* a_idx, const double* b, const long long* b_idx, int n,
                               double* out, cudaStream_t st) {
   if (n == 0) return cudaSuccess;
-  pc_abs_dot_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, a_idx, b, b_idx, n, out);
-  return cudaGetLastError();
+  return launch(pc_abs_dot_kernel, (n + 255) / 256, 256, 0, st, false, a, a_idx, b, b_idx, n, out);
 }
 
 cudaError_t launch_f64_mean(const double* x, int n, double* out, void* workspace, cudaStream_t st) {
   double* part = reinterpret_cast<double*>(static_cast<uint8_t*>(workspace) + al256(sizeof(SelState)) + al256(256 * 4));
-  f64_sum_kernel<<<RED_BLOCKS, RED_T, 0, st>>>(x, n, part);
-  f64_mean_final_kernel<<<1, 32, 0, st>>>(part, n, out);
-  return cudaGetLastError();
+  const cudaError_t e = launch(f64_sum_kernel, RED_BLOCKS, RED_T, 0, st, false, x, n, part);
+  if (e != cudaSuccess) return e;
+  return launch(f64_mean_final_kernel, 1, 32, 0, st, false, part, n, out);
 }
 
-cudaError_t launch_f64_median(const double* x, int n, double* out, void* workspace, cudaStream_t st, int* launches) {
+cudaError_t launch_f64_median(const double* x, int n, double* out, void* workspace, cudaStream_t st) {
   SelState* s = static_cast<SelState*>(workspace);
   uint32_t* hist = reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(workspace) + al256(sizeof(SelState)));
   const int k = (n - 1) / 2;  // odd n: the middle; even n: the lower middle, its successor below
   const int g = min(1024, (n + RED_T - 1) / RED_T);
-  sel_init_kernel<<<1, 256, 0, st>>>(s, hist, k);
+  cudaError_t e;
+  if ((e = launch(sel_init_kernel, 1, 256, 0, st, false, s, hist, k)) != cudaSuccess) return e;
   for (int shift = 56; shift >= 0; shift -= 8) {
-    sel_hist_kernel<<<g, RED_T, 0, st>>>(x, n, s, hist, shift);
-    sel_digit_kernel<<<1, 256, 0, st>>>(s, hist, shift);
+    if ((e = launch(sel_hist_kernel, g, RED_T, 0, st, false, x, n, s, hist, shift)) != cudaSuccess) return e;
+    if ((e = launch(sel_digit_kernel, 1, 256, 0, st, false, s, hist, shift)) != cudaSuccess) return e;
   }
-  if (!(n & 1)) sel_succ_kernel<<<g, RED_T, 0, st>>>(x, n, s);
-  sel_final_kernel<<<1, 32, 0, st>>>(s, n, out);
-  *launches = 2 + 16 + !(n & 1);
-  return cudaGetLastError();
+  if (!(n & 1) && (e = launch(sel_succ_kernel, g, RED_T, 0, st, false, x, n, s)) != cudaSuccess) return e;
+  return launch(sel_final_kernel, 1, 32, 0, st, false, s, n, out);
 }
 
 cudaError_t launch_f64_count_below(const double* x, int n, const double* th, unsigned long long* count, cudaStream_t st) {
   cudaError_t e = cudaMemsetAsync(count, 0, sizeof(unsigned long long), st);
   if (e != cudaSuccess || n == 0) return e;
-  f64_count_below_kernel<<<min(1024, (n + RED_T - 1) / RED_T), RED_T, 0, st>>>(x, n, th, count);
-  return cudaGetLastError();
+  return launch(f64_count_below_kernel, min(1024, (n + RED_T - 1) / RED_T), RED_T, 0, st, false, x, n, th, count);
 }
 
 }  // namespace f3r
