@@ -8,6 +8,7 @@
 
 #include "../../include/fast3r_b200.h"
 #include "f3r_kernels.h"
+#include "gemm_plan.h"
 
 namespace {
 
@@ -104,32 +105,22 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
   if (d->epi == F3R_EPI_IDXEMB && (!d->emb_table || !d->emb_ids || d->tok_per_img < 0))
     return fail("f3r_gemm: bad IDXEMB arguments");
 
+  static int dbg = -1, tma_pref = -1, ksplit_pref = -1;
+  if (dbg < 0) { const char* e = getenv("F3R_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }
+  if (tma_pref < 0) { const char* e = getenv("F3R_GEMM_TMA_EPI"); tma_pref = (e && e[0] == '0') ? 0 : 1; }
+  // F3R_GEMM_KSPLIT=1 disables the K slicing (A/B measurements)
+  if (ksplit_pref < 0) { const char* e = getenv("F3R_GEMM_KSPLIT"); ksplit_pref = (e && e[0] == '1') ? 1 : 0; }
+  const f3r::GemmPlan plan = f3r::gemm_plan(*d, num_sms(), tma_pref, ksplit_pref != 1);
+  const int block_n = plan.block_n;
+
   f3r::GemmArgs a;
   memset(&a, 0, sizeof(a));
   a.M = d->w * d->h * d->nb; a.N = d->n; a.K = d->k; a.taps = d->taps;
   a.W = d->w; a.H = d->h; a.NB = d->nb;
-  // pixel tile (bw x bh = 128) minimising the number of tiles
-  int best_bw = 128; long best_tiles = -1;
-  for (int bw = 128; bw >= 1; bw >>= 1) {
-    const int bh = 128 / bw;
-    const long tiles = static_cast<long>((d->w + bw - 1) / bw) * ((d->h + bh - 1) / bh);
-    if (best_tiles < 0 || tiles < best_tiles) { best_tiles = tiles; best_bw = bw; }
-  }
-  a.bw = best_bw; a.bh = 128 / best_bw;
-  a.bw_log2 = 0;
-  while ((1 << a.bw_log2) < a.bw) ++a.bw_log2;
-  a.sbx_log2 = a.bw_log2 < 5 ? a.bw_log2 : 5;
-  a.tiles_x = (d->w + a.bw - 1) / a.bw; a.tiles_y = (d->h + a.bh - 1) / a.bh;
-  a.num_m_tiles = a.tiles_x * a.tiles_y * d->nb;
-  int block_n = 128;
-  if (d->epi != F3R_EPI_FINAL && d->n > 128) {
-    const long tiles256 = static_cast<long>(a.num_m_tiles) * ((d->n + 255) / 256);
-    if (tiles256 >= num_sms()) block_n = 256;
-  }
-  a.num_n_tiles = (d->n + block_n - 1) / block_n;
-  static int dbg = -1, tma_pref = -1;
-  if (dbg < 0) { const char* e = getenv("F3R_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }
-  if (tma_pref < 0) { const char* e = getenv("F3R_GEMM_TMA_EPI"); tma_pref = (e && e[0] == '0') ? 0 : 1; }
+  a.bw = plan.bw; a.bh = plan.bh; a.bw_log2 = plan.bw_log2; a.sbx_log2 = plan.sbx_log2;
+  a.tiles_x = plan.tiles_x; a.tiles_y = plan.tiles_y; a.num_m_tiles = plan.num_m_tiles;
+  a.num_n_tiles = plan.num_n_tiles;
+  a.tma_epi = plan.tma_epi; a.k_split = plan.k_split;
   a.debug = dbg;
   a.epi = d->epi; a.act = d->act; a.out0_f32 = d->out0_f32; a.res0_f32 = d->res0_f32;
   a.ldo = d->ldo > 0 ? d->ldo : d->n;
@@ -159,14 +150,10 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
     const uint32_t box[3] = {64, 1, static_cast<uint32_t>(block_n)};
     if (make_tmap(&tb, d->wt, 3, dims, str, box)) return 1;
   }
-  // TMA epilogue for the hot cases: plain (activated) stores, and the in-place fp32 residual update as a reduce-add
+  // output tensor maps of the TMA epilogue (plan.tma_epi: plain stores, or the in-place fp32 residual reduce-add)
   CUtensorMap to0, to0b;
   memset(&to0, 0, sizeof(to0));
   memset(&to0b, 0, sizeof(to0b));
-  const bool plain = (d->epi == F3R_EPI_STORE || d->epi == F3R_EPI_ROPE || d->epi == F3R_EPI_IDXEMB) && d->out0 &&
-                     !d->out1 && !d->res1;
-  if (tma_pref && plain && !d->res0) a.tma_epi = 1;
-  else if (tma_pref && plain && d->res0 == d->out0 && d->res0_f32 && d->out0_f32 && !d->split_col) a.tma_epi = 2;
   if (a.tma_epi) {
     const uint64_t es = d->out0_f32 ? 4 : 2;
     const CUtensorMapDataType dt = d->out0_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
@@ -187,20 +174,6 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
                                 static_cast<uint64_t>(d->h), static_cast<uint64_t>(d->nb)};
       const uint64_t str[3] = {ld, ld * d->w, ld * d->w * d->h};
       if (make_tmap(&to0b, d->out0b, 4, dims, str, box, dt, sw)) return 1;
-    }
-  }
-  a.k_split = 1;
-  static int ksplit_pref = -1;  // F3R_GEMM_KSPLIT=1 disables the K slicing (A/B measurements)
-  if (ksplit_pref < 0) { const char* e = getenv("F3R_GEMM_KSPLIT"); ksplit_pref = (e && e[0] == '1') ? 1 : 0; }
-  if (a.tma_epi == 2 && d->taps == 1 && ksplit_pref != 1) {
-    // x += A W^T with fewer output tiles than SMs: cut K into slices, each CTA reduce-adds its partial sum
-    const long slots = num_sms();
-    const long items = static_cast<long>(a.num_m_tiles) * a.num_n_tiles;
-    const int k_iters = (d->k + 63) / 64;
-    double best = 1e30;
-    for (int s = 1; s <= 4 && (s == 1 || k_iters / s >= 16); ++s) {  // (short K: the reduce-add epilogue dominates, slicing loses)
-      const double cost = static_cast<double>((items * s + slots - 1) / slots) / s * (1.0 + 0.03 * (s - 1));
-      if (cost < best - 1e-9) { best = cost; a.k_split = s; }
     }
   }
   return check(f3r::launch_gemm(block_n, ta, tb, to0, to0b, a, num_sms(), static_cast<cudaStream_t>(stream)),

@@ -1,5 +1,5 @@
 """Per-kernel numerics checks: each CUDA op (through the C ABI) against a plain PyTorch fp32 reference of the
-same op on the same bf16-rounded operands.  Used by tests/test_kernels_gpu.py (asserting) and by
+same op on the same bf16-rounded operands (the GEMM cases: per element against float64, tests/test_gemm_plans_gpu.py).  Used by tests/test_kernels_gpu.py (asserting) and by
 tools/gpu_check.py (report-everything mode for debugging on the GPU box)."""
 import math
 
@@ -20,134 +20,16 @@ def _rand(shape, seed, scale=1.0, dtype=torch.bfloat16):
     return (torch.randn(shape, generator=g) * scale).to(dtype).cuda()
 
 
-def check_linear(M=300, K=192, N=96, seed=0):
-    a, w = _rand((M, K), seed), _rand((N, K), seed + 1, K ** -0.5)
-    bias = _rand((N,), seed + 2, 1.0, torch.float32)
-    out = torch.zeros(M, N, dtype=torch.bfloat16, device="cuda")
-    ops.linear(a, w, bias, out0=out)
-    ref = a.float() @ w.float().T + bias
-    return rel(out, ref), 6e-3, dict(max_abs=float((out.float() - ref).abs().max()))
-
-
-def check_linear_f32_residual_gelu(M=1000, K=1024, N=512, seed=10):
-    a, w = _rand((M, K), seed), _rand((N, K), seed + 1, K ** -0.5)
-    bias = _rand((N,), seed + 2, 1.0, torch.float32)
-    x = _rand((M, N), seed + 3, 1.0, torch.float32)
-    x0 = x.clone()
-    ops.linear(a, w, bias, out0=x, res0=x)  # in-place fp32 residual update
-    ref = x0 + a.float() @ w.float().T + bias
-    e1 = rel(x, ref)
-    g = torch.zeros(M, N, dtype=torch.bfloat16, device="cuda")
-    r = torch.zeros(M, N, dtype=torch.bfloat16, device="cuda")
-    ops.linear(a, w, bias, out0=g, out1=r, act=L.ACT_GELU)
-    ref0 = a.float() @ w.float().T + bias
-    e2 = rel(g, F.gelu(ref0))
-    e3 = rel(r, F.relu(ref0))
-    return max(e1 * 1000, e2, e3), 6e-3, dict(resid_f32=e1, gelu=e2, relu_copy=e3)
-
-
-def check_linear_split(M=520, K=128, D=128, seed=20):
-    a, w = _rand((M, K), seed), _rand((3 * D, K), seed + 1, K ** -0.5)
-    bias = _rand((3 * D,), seed + 2, 1.0, torch.float32)
-    q = torch.zeros(M, D, dtype=torch.bfloat16, device="cuda")
-    kv = torch.zeros(M, 2 * D, dtype=torch.bfloat16, device="cuda")
-    ops.linear(a, w, bias, out0=q, ldo=D, split_col=D, out0b=kv, ldo_b=2 * D)
-    ref = a.float() @ w.float().T + bias
-    return max(rel(q, ref[:, :D]), rel(kv, ref[:, D:])), 6e-3, {}
-
-
-def rope_tables(max_pos, base=100.0):
-    j = torch.arange(16, dtype=torch.float32)
-    inv = 1.0 / (base ** (j / 16.0))
-    ang = torch.arange(max_pos, dtype=torch.float32)[:, None] * inv[None]
-    return ang.cos().contiguous().cuda(), ang.sin().contiguous().cuda()
-
-
-def check_rope(n_img=3, gh=5, gw=8, heads=2, seed=30):
-    from oracle.fast3r_oracle import rope2d
-    D = heads * 64
-    P = gh * gw
-    M = n_img * P
-    a, w = _rand((M, D), seed), _rand((3 * D, D), seed + 1, D ** -0.5)
-    bias = _rand((3 * D,), seed + 2, 1.0, torch.float32)
-    out = torch.zeros(M, 3 * D, dtype=torch.bfloat16, device="cuda")
-    cos, sin = rope_tables(max(gh, gw))
-    ops.linear(a, w, bias, out0=out, epi=L.EPI_ROPE, tok_per_img=P, grid_w=gw, rope_cols=2 * D, rope_cos=cos,
-               rope_sin=sin)
-    ref = (a.float() @ w.float().T + bias).cpu().reshape(n_img, P, 3, heads, 64).permute(2, 0, 3, 1, 4)
-    yy, xx = torch.meshgrid(torch.arange(gh), torch.arange(gw), indexing="ij")
-    pos = torch.stack((yy.reshape(-1), xx.reshape(-1)), -1)[None].expand(n_img, -1, -1)
-    qr, kr = rope2d(ref[0], pos), rope2d(ref[1], pos)
-    ref = torch.stack((qr, kr, ref[2])).permute(1, 3, 0, 2, 4).reshape(M, 3 * D)
-    return rel(out.cpu(), ref), 6e-3, {}
-
-
-def check_idxemb(B=2, N=3, P=24, D=128, seed=40):
-    M = B * N * P
-    a, w = _rand((M, D), seed), _rand((D, D), seed + 1, D ** -0.5)
-    bias = _rand((D,), seed + 2, 1.0, torch.float32)
-    table = _rand((1000, D), seed + 3, 1.0, torch.float32)
-    ids = torch.tensor([[0, 5, 999], [0, 17, 3]], dtype=torch.int32).cuda()
-    out = torch.zeros(M, D, dtype=torch.float32, device="cuda")
-    ops.linear(a, w, bias, out0=out, epi=L.EPI_IDXEMB, tok_per_img=P, emb_table=table, emb_ids=ids)
-    ref = a.float() @ w.float().T + bias + table[ids.long().flatten()].repeat_interleave(P, 0)
-    return rel(out, ref) * 100, 6e-3, dict(rel=rel(out, ref))
-
-
-def check_conv3x3(nb=2, H=20, W=256, C=64, N=128, seed=50, res=False):
-    x = _rand((nb, H, W, C), seed)
-    w = _rand((N, C, 3, 3), seed + 1, (9 * C) ** -0.5)
-    bias = _rand((N,), seed + 2, 1.0, torch.float32)
-    wt = w.permute(0, 2, 3, 1).reshape(N, 9, C).contiguous()
-    out = torch.zeros(nb, H, W, N, dtype=torch.bfloat16, device="cuda")
-    out1 = torch.zeros_like(out)
-    kw = {}
-    ref = F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), bias, padding=1).permute(0, 2, 3, 1)
-    if res:
-        r0, r1 = _rand((nb, H, W, N), seed + 3), _rand((nb, H, W, N), seed + 4)
-        kw = dict(res0=r0, res1=r1)
-        ref = ref + r0.float() + r1.float()
-    ops.gemm(x, wt, w=W, h=H, nb=nb, taps=9, bias=bias, out0=out, out1=out1, **kw)
-    return max(rel(out, ref), rel(out1, F.relu(ref))), 6e-3, {}
-
-
-def check_conv1x1(nb=3, H=4, W=6, C=128, N=96, seed=60):
-    x = _rand((nb, H, W, C), seed)
-    w = _rand((N, C), seed + 1, C ** -0.5)
-    bias = _rand((N,), seed + 2, 1.0, torch.float32)
-    out = torch.zeros(nb, H, W, N, dtype=torch.bfloat16, device="cuda")
-    ops.gemm(x, w.reshape(N, 1, C), w=W, h=H, nb=nb, bias=bias, out0=out)
-    ref = x.float() @ w.float().T + bias
-    return rel(out, ref), 6e-3, {}
-
-
-def check_convt(nb=2, H=4, W=6, C=96, k=4, seed=70):
-    x = _rand((nb, H, W, C), seed)
-    w = _rand((C, C, k, k), seed + 1, C ** -0.5)  # ConvTranspose2d weight (in, out, kh, kw)
-    bias = _rand((C,), seed + 2, 1.0, torch.float32)
-    wt = w.permute(2, 3, 1, 0).reshape(k * k * C, 1, C).contiguous()  # ((i*k+j)*out + o, in)
-    out = torch.zeros(nb, H * k, W * k, C, dtype=torch.bfloat16, device="cuda")
-    ops.gemm(x, wt, w=W, h=H, nb=nb, bias=bias, out0=out, epi=L.EPI_CONVT, ct_k=k, ct_cout=C)
-    ref = F.conv_transpose2d(x.float().permute(0, 3, 1, 2), w.float(), bias, stride=k).permute(0, 2, 3, 1)
-    return rel(out, ref), 6e-3, {}
-
-
-def check_final(nb=2, H=16, W=96, C=128, seed=80):
-    x = _rand((nb, H, W, C), seed)
-    w = _rand((128, C, 3, 3), seed + 1, (9 * C) ** -0.5)
-    bias = _rand((128,), seed + 2, 0.5, torch.float32)
-    w4 = _rand((4, 128), seed + 3, 128 ** -0.5, torch.float32)
-    b4 = _rand((4,), seed + 4, 0.5, torch.float32)
-    wt = w.permute(0, 2, 3, 1).reshape(128, 9, C).contiguous()
-    pts = torch.zeros(nb, H, W, 3, dtype=torch.float32, device="cuda")
-    conf = torch.zeros(nb, H, W, dtype=torch.float32, device="cuda")
-    ops.gemm(x, wt, w=W, h=H, nb=nb, taps=9, bias=bias, epi=L.EPI_FINAL, w4=w4, b4=b4, pts=pts, conf=conf)
-    y = F.relu(F.conv2d(x.float().permute(0, 3, 1, 2), w.float(), bias, padding=1)).permute(0, 2, 3, 1)
-    o = y @ w4.T + b4
-    d = o[..., :3].norm(dim=-1, keepdim=True)
-    rp = o[..., :3] / d.clip(min=1e-8) * torch.expm1(d)
-    rc = 1 + o[..., 3].exp()
-    return max(rel(pts, rp), rel(conf, rc)), 2e-3, dict(pts=rel(pts, rp), conf=rel(conf, rc))
+def check_gemm(names):
+    """The GEMM cases `names` of tests/gemm_plans.CASES, each checked per element against float64 and for its launch
+    plan (tests/test_gemm_plans_gpu.run_case; it raises on a failure)."""
+    from tests import gemm_plans as GP
+    from tests.test_gemm_plans_gpu import run_case
+    for name in names:
+        i, case = next((i, c) for i, c in enumerate(GP.CASES) if c["name"] == name)
+        assert GP.plan_key(case) == case["key"], (name, GP.plan_key(case), case["key"])
+        run_case(case, seed=1000 + i)
+    return 0.0, 0.0, {}
 
 
 def attention_ref(q, k, v, scale):
@@ -383,22 +265,22 @@ ALL = [
     ("im2col3x3s2", check_im2col3x3s2, {}),
     ("upsample_crop", check_upsample, {}),
     ("upsample_full", check_upsample, dict(H=23, W=32, C=128, crop=False)),
-    ("linear_small_tails", check_linear, {}),
-    ("linear_qkv_shape", check_linear, dict(M=2944, K=1024, N=3072)),
-    ("linear_bn256", check_linear, dict(M=23552, K=256, N=1024)),
-    ("linear_resid_gelu", check_linear_f32_residual_gelu, {}),
-    ("linear_resid_splitk", check_linear_f32_residual_gelu, dict(M=300, K=4096, N=256)),  # K slices reduce-added into x
-    ("linear_split", check_linear_split, {}),
-    ("rope_epilogue", check_rope, {}),
-    ("idxemb_epilogue", check_idxemb, {}),
-    ("conv1x1_tinymap", check_conv1x1, {}),
-    ("conv3x3_w256", check_conv3x3, {}),
-    ("conv3x3_w6_c96_res", check_conv3x3, dict(nb=3, H=4, W=6, C=96, N=256, res=True)),
-    ("conv3x3_w24_c192", check_conv3x3, dict(nb=1, H=16, W=24, C=192, N=256)),
-    ("conv3x3_w512", check_conv3x3, dict(nb=1, H=40, W=512, C=128, N=128)),
-    ("convT_k4", check_convt, {}),
-    ("convT_k2", check_convt, dict(C=192, k=2)),
-    ("final_fused", check_final, {}),
+    ("linear_small_tails", check_gemm, dict(names=["linear_small_tails"])),
+    ("linear_qkv_shape", check_gemm, dict(names=["linear_qkv_shape"])),
+    ("linear_bn256", check_gemm, dict(names=["linear_bn256"])),
+    ("linear_resid_gelu", check_gemm, dict(names=["linear_resid_gelu", "linear_resid_gelu_out1"])),
+    ("linear_resid_splitk", check_gemm, dict(names=["linear_resid_splitk", "linear_resid_splitk_out1"])),  # K slices
+    ("linear_split", check_gemm, dict(names=["linear_split"])),
+    ("rope_epilogue", check_gemm, dict(names=["rope_epilogue"])),
+    ("idxemb_epilogue", check_gemm, dict(names=["idxemb_epilogue"])),
+    ("conv1x1_tinymap", check_gemm, dict(names=["conv1x1_tinymap"])),
+    ("conv3x3_w256", check_gemm, dict(names=["conv3x3_w256"])),
+    ("conv3x3_w6_c96_res", check_gemm, dict(names=["conv3x3_w6_c96_res"])),
+    ("conv3x3_w24_c192", check_gemm, dict(names=["conv3x3_w24_c192"])),
+    ("conv3x3_w512", check_gemm, dict(names=["conv3x3_w512"])),
+    ("convT_k4", check_gemm, dict(names=["convT_k4"])),
+    ("convT_k2", check_gemm, dict(names=["convT_k2"])),
+    ("final_fused", check_gemm, dict(names=["final_fused"])),
     ("attn_736_b2h2", check_attention, {}),
     ("attn_128", check_attention, dict(batch=1, heads=1, sq=128, skv=128)),
     ("attn_256x384", check_attention, dict(batch=1, heads=2, sq=256, skv=384)),
