@@ -19,6 +19,8 @@
 // with two consumer warpgroups.
 // The arithmetic (ex2 inputs, order of the l and O updates, lazy-rescale decisions) is that of a loop that finishes one
 // key block before it starts the next, so the overlap does not change a bit of the result.
+// Segment mode (attention_kernel<true>, f3r_attention_segments): block-diagonal attention over the segments of one packed
+// sequence, each segment with the arithmetic of a launch over it alone.
 #include "common.cuh"
 #include "f3r_kernels.h"
 
@@ -111,6 +113,43 @@ F3R_DEVICE void att_rescale_pack(float (&o)[32], uint32_t (&pa)[8][4], const flo
     for (int r = 0; r < 4; ++r) pa[kk][r] = pack_bf16(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
 }
 
+// Segment mode: finds the segment of work item `item`.  Items are numbered segment by segment, heads * n_split per query
+// tile of the segment; the warp scans the segments' query-tile counts 32 at a time.  Returns false past the last item
+// (the grid is sized by an upper bound of the tile count).  local: the item's index inside its segment.
+F3R_DEVICE bool att_find_segment(const AttnArgs& p, int item, int& s0, int& len, int& local) {
+  const int lane = threadIdx.x & 31;
+  const int per_tile = p.heads * p.n_split;
+  const int tile = item / per_tile;  // query tile of the item, counted over all segments
+  int base = 0;                      // query tiles of the segments before this step's first
+  for (int c = 0; c < p.n_seg; c += 32) {
+    const int i = c + lane;
+    const int t = i < p.n_seg ? (max(__ldg(p.seg_off + i + 1) - __ldg(p.seg_off + i), 0) + ATT_Q_TILE - 1) / ATT_Q_TILE : 0;
+    int incl = t;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += y;
+    }
+    const unsigned hit = __ballot_sync(0xffffffffu, base + incl > tile);
+    if (hit) {
+      const int l = __ffs(hit) - 1;
+      const int before = base + __shfl_sync(0xffffffffu, incl - t, l);
+      s0 = __ldg(p.seg_off + c + l);
+      len = __ldg(p.seg_off + c + l + 1) - s0;  // > 0: the segment has a query tile
+      local = item - before * per_tile;
+      return true;
+    }
+    base += __shfl_sync(0xffffffffu, incl, 31);
+  }
+  return false;
+}
+
+// kSeg = false: p.batch independent sequences of p.sq queries / p.skv keys.
+// kSeg = true: one packed sequence of p.sq rows cut into p.n_seg segments (p.seg_off); each segment attends to its own
+// rows only, with key blocks that start at its first row, so its rows get exactly the arithmetic of a kSeg = false launch
+// over that segment alone.  A segment with fewer key blocks than p.n_split uses one slice per key block and fills the
+// slots of its other slices with neutral partials (O = 0, LSE = -inf: merge weight 0).
+template <bool kSeg>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
                  const __grid_constant__ AttnArgs p) {
@@ -129,17 +168,18 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // work item = (unit = (batch, head, query tile of ATT_Q_TILE rows), split = slice of the key blocks of this launch's
-  // key range)
-  const int unit = blockIdx.x / p.n_split;
-  const int split = blockIdx.x % p.n_split;
-  const int qt = unit % p.q_tiles;
-  const int bh = unit / p.q_tiles;
-  const int h = bh % p.heads;
-  const int b = bh / p.heads;
-  const int nkv_all = (p.skv + 127) / 128;
-  const int j0 = static_cast<int>(static_cast<long long>(split) * nkv_all / p.n_split);  // first key block of this CTA
-  const int nkv = static_cast<int>(static_cast<long long>(split + 1) * nkv_all / p.n_split) - j0;  // (>= 1, host-checked)
+  // work item = (unit = (batch or segment, head, query tile of ATT_Q_TILE rows), split = slice of the key blocks of the
+  // unit's key range).  sq / skv: queries / keys of the unit; s0: its first row in the packed sequence (segment mode)
+  int split, qt, h, b, sq, skv, n_split, s0 = 0, kv_row0 = p.kv_row0;
+  if constexpr (!kSeg) {
+    const int unit = blockIdx.x / p.n_split;
+    split = blockIdx.x % p.n_split;
+    qt = unit % p.q_tiles;
+    const int bh = unit / p.q_tiles;
+    h = bh % p.heads;
+    b = bh / p.heads;
+    sq = p.sq; skv = p.skv; n_split = p.n_split;
+  }
   const int dmodel = p.heads * 64;
 
   if (threadIdx.x == 0) {
@@ -156,22 +196,51 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   pdl_wait();                // q / kv come from the preceding QKV GEMM: no global access above this line
   pdl_launch_dependents();
 
+  if constexpr (kSeg) {
+    int local;
+    if (!att_find_segment(p, blockIdx.x, s0, sq, local)) return;
+    skv = sq;
+    kv_row0 = s0;
+    b = 0;
+    split = local % p.n_split;
+    const int unit = local / p.n_split;
+    const int q_tiles = (sq + ATT_Q_TILE - 1) / ATT_Q_TILE;
+    qt = unit % q_tiles;
+    h = unit / q_tiles;
+    n_split = min(p.n_split, (skv + 127) / 128);
+    if (split >= n_split) {
+      // no key block left for this slice (only with part_o, host-checked): a neutral partial for the merge
+      const size_t slot = static_cast<size_t>(p.part_base + split);
+      const int q0 = s0 + qt * ATT_Q_TILE, rows = min(ATT_Q_TILE, sq - qt * ATT_Q_TILE);
+      for (int i = threadIdx.x; i < rows * 16; i += ATT_THREADS)
+        *reinterpret_cast<float4*>(p.part_o + (slot * p.sq + q0 + (i >> 4)) * dmodel + h * 64 + 4 * (i & 15)) =
+            make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int i = threadIdx.x; i < rows; i += ATT_THREADS)
+        p.part_lse[(slot * p.heads + h) * p.sq + q0 + i] = -INFINITY;
+      return;
+    }
+  }
+  const int nkv_all = (skv + 127) / 128;
+  const int j0 = static_cast<int>(static_cast<long long>(split) * nkv_all / n_split);  // first key block of this CTA
+  const int nkv = static_cast<int>(static_cast<long long>(split + 1) * nkv_all / n_split) - j0;  // (>= 1, host-checked)
+
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");   // 128 x 24 + 384 x 160 <= 64K registers
     if (warp == 0 && lane == 0) {
       // ===================== TMA producer =====================
       // (Q rows past sq are zero-filled by the TMA unit and still count towards the transaction bytes)
       mbar_arrive_expect_tx(q_full, ATT_Q_BYTES);
-      tma_load_3d(smem_q, &tmap_q, q_full, h * 64, qt * ATT_Q_TILE, b);
+      // (segment mode: the Q rows past the segment are the next segment's; they are computed and never stored)
+      tma_load_3d(smem_q, &tmap_q, q_full, h * 64, s0 + qt * ATT_Q_TILE, b);
       int stage = 0; uint32_t phase = 0;
       for (int j = 0; j < nkv; ++j) {
         mbar_wait_relaxed(&k_empty[stage], phase ^ 1);
         mbar_arrive_expect_tx(&k_full[stage], ATT_TILE_BYTES);
-        tma_load_3d(smem_k + stage * ATT_TILE_BYTES, &tmap_kv, &k_full[stage], h * 64, p.kv_row0 + (j0 + j) * 128, b);
+        tma_load_3d(smem_k + stage * ATT_TILE_BYTES, &tmap_kv, &k_full[stage], h * 64, kv_row0 + (j0 + j) * 128, b);
         mbar_wait_relaxed(&v_empty[stage], phase ^ 1);
         mbar_arrive_expect_tx(&v_full[stage], ATT_TILE_BYTES);
         tma_load_3d(smem_v + stage * ATT_TILE_BYTES, &tmap_kv, &v_full[stage], dmodel + h * 64,
-                    p.kv_row0 + (j0 + j) * 128, b);
+                    kv_row0 + (j0 + j) * 128, b);
         if (++stage == ATT_STAGES) { stage = 0; phase ^= 1; }
       }
     }
@@ -196,7 +265,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     float alpha[2];      // ... and its factor
     const uint64_t qd = make_smem_desc_sw128(smem_u32(smem_q + cg * 64 * 128));
     // keys valid in key block j of this CTA: only the last block of the launch's key range is partial
-    auto valid_keys = [&](int j) { return j0 + j == nkv_all - 1 ? p.skv - (j0 + j) * 128 : 128; };
+    auto valid_keys = [&](int j) { return j0 + j == nkv_all - 1 ? skv - (j0 + j) * 128 : 128; };
     mbar_wait(q_full, 0);
 
     // block 0: S_0 and its softmax
@@ -233,6 +302,18 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     {
       const int sv = (nkv - 1) % ATT_STAGES;
       mbar_wait(&v_full[sv], ((nkv - 1) / ATT_STAGES) & 1);
+      if constexpr (kSeg) {
+        // The V rows past the segment's end belong to the next segment.  Their scores are masked, but P = 0 times a NaN
+        // or Inf in V would still reach O, so they enter the PV product as zeros, as the TMA zero fill gives a single-
+        // segment launch.  A 128B-swizzled row stays within its own 128 bytes, so whole rows are zeroed.
+        const int valid = valid_keys(nkv - 1);
+        if (valid < 128) {
+          uint4* v4 = reinterpret_cast<uint4*>(smem_v + sv * ATT_TILE_BYTES + valid * 128);
+          for (int i = threadIdx.x - 128; i < (128 - valid) * 8; i += 128 * ATT_CONSUMERS) v4[i] = make_uint4(0, 0, 0, 0);
+          fence_proxy_async_smem();  // generic-proxy stores before the wgmma (async proxy) reads
+          asm volatile("bar.sync 1, %0;" ::"n"(128 * ATT_CONSUMERS) : "memory");  // all consumer warpgroups
+        }
+      }
       wgmma_wait<0>();
       fence_regs(o);
       if (nkv > 1 && wg_tid == 0) mbar_arrive(&v_empty[(nkv - 2) % ATT_STAGES]);
@@ -253,30 +334,38 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int q = qt * ATT_Q_TILE + rw + 8 * hh;
-      if (q >= p.sq) continue;
+      if (q >= sq) continue;
+      const int qs = kSeg ? s0 + q : q;  // row in the per-batch sequence of p.sq rows
+      if (kSeg && qs >= p.sq) continue;  // (segment offsets past the buffer)
       const float inv = 1.f / l[hh];
       const float lse = m_used[hh] * sl2 * 0.69314718056f + logf(l[hh]);
       if (p.part_o != nullptr) {
         // partial result of this key slice: normalised fp32 O and its log-sum-exp; f3r_attention_merge combines slices
         const size_t slot = static_cast<size_t>(p.part_base + split);
-        float* dstf = p.part_o + (slot * p.batch * p.sq + static_cast<size_t>(b) * p.sq + q) * dmodel + h * 64 + cq;
+        float* dstf = p.part_o + (slot * p.batch * p.sq + static_cast<size_t>(b) * p.sq + qs) * dmodel + h * 64 + cq;
 #pragma unroll
         for (int jn = 0; jn < 8; ++jn)
           *reinterpret_cast<float2*>(dstf + 8 * jn) = make_float2(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv);
-        if ((lane & 3) == 0) p.part_lse[(slot * p.batch * p.heads + static_cast<size_t>(b) * p.heads + h) * p.sq + q] = lse;
+        if ((lane & 3) == 0) p.part_lse[(slot * p.batch * p.heads + static_cast<size_t>(b) * p.heads + h) * p.sq + qs] = lse;
       } else {
-        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.out) + (static_cast<size_t>(b) * p.sq + q) * p.ldo + h * 64 + cq;
+        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.out) + (static_cast<size_t>(b) * p.sq + qs) * p.ldo + h * 64 + cq;
 #pragma unroll
         for (int jn = 0; jn < 8; ++jn)
           *reinterpret_cast<uint32_t*>(dst + 8 * jn) = pack_bf16(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv);
-        if (p.lse != nullptr && (lane & 3) == 0) p.lse[(static_cast<size_t>(b) * p.heads + h) * p.sq + q] = lse;
+        if (p.lse != nullptr && (lane & 3) == 0) p.lse[(static_cast<size_t>(b) * p.heads + h) * p.sq + qs] = lse;
       }
     }
   }
 }
 
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, cudaStream_t stream) {
-  return launch(attention_kernel, a.batch * a.heads * a.q_tiles * a.n_split, ATT_THREADS, ATT_SMEM_BYTES, stream, true, tq,
+  return launch(attention_kernel<false>, a.batch * a.heads * a.q_tiles * a.n_split, ATT_THREADS, ATT_SMEM_BYTES, stream,
+                true, tq, tkv, a);
+}
+
+cudaError_t launch_attention_segments(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, int max_tiles,
+                                      cudaStream_t stream) {
+  return launch(attention_kernel<true>, a.heads * a.n_split * max_tiles, ATT_THREADS, ATT_SMEM_BYTES, stream, true, tq,
                 tkv, a);
 }
 

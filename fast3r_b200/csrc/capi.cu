@@ -233,6 +233,49 @@ int f3r_attention_partial(const void* q, int32_t ldq, const void* kv, int32_t ld
                         part_lse, part_base, n_split, batch, heads, sq, skv, scale, stream);
 }
 
+int f3r_attention_segments(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo,
+                           const int32_t* seg_off, int32_t n_seg, int32_t rows, int32_t heads, float scale,
+                           int32_t n_split, float* part_o, float* part_lse, void* stream) {
+  const char* what = "f3r_attention_segments";
+  if (!q || !kv || !seg_off) return fail("%s: null operand", what);
+  if (reinterpret_cast<uintptr_t>(seg_off) & 3) return fail("%s: seg_off not 4-byte aligned", what);
+  if (n_seg <= 0 || rows <= 0 || heads <= 0) return fail("%s: bad shape", what);
+  if (ldq % 8 || ldkv % 8 || ldq < heads * 64 || ldkv < 2 * heads * 64) return fail("%s: bad leading dimensions", what);
+  if (n_split < 1 || n_split > (rows + 127) / 128) return fail("%s: n_split=%d must be in [1, #key blocks]", what, n_split);
+  if (!part_o != !part_lse) return fail("%s: part_o and part_lse must be given together", what);
+  if (!part_o) {
+    if (n_split != 1) return fail("%s: n_split > 1 writes key-slice partials: part_o / part_lse needed", what);
+    if (!out) return fail("%s: null operand", what);
+    if (ldo % 8 || ldo < heads * 64) return fail("%s: bad leading dimensions", what);
+  }
+  // sum over segments of ceil(len / ATT_Q_TILE) <= (rows + (ATT_Q_TILE - 1) * n_seg) / ATT_Q_TILE; the CTAs past the
+  // last work item exit at once
+  const long long max_tiles = (rows + static_cast<long long>(f3r::ATT_Q_TILE - 1) * n_seg) / f3r::ATT_Q_TILE;
+  if (max_tiles * heads * n_split > 0x7fffffffLL) return fail("%s: too many work items", what);
+  CUtensorMap tq, tkv;
+  {
+    const uint64_t dims[3] = {static_cast<uint64_t>(heads) * 64, static_cast<uint64_t>(rows), 1};
+    const uint64_t str[2] = {static_cast<uint64_t>(ldq) * 2, static_cast<uint64_t>(ldq) * 2 * rows};
+    const uint32_t box[3] = {64, f3r::ATT_Q_TILE, 1};
+    if (make_tmap(&tq, q, 3, dims, str, box)) return 1;
+  }
+  {
+    const uint64_t dims[3] = {static_cast<uint64_t>(heads) * 128, static_cast<uint64_t>(rows), 1};
+    const uint64_t str[2] = {static_cast<uint64_t>(ldkv) * 2, static_cast<uint64_t>(ldkv) * 2 * rows};
+    const uint32_t box[3] = {64, 128, 1};
+    if (make_tmap(&tkv, kv, 3, dims, str, box)) return 1;
+  }
+  f3r::AttnArgs a;
+  memset(&a, 0, sizeof(a));
+  a.batch = 1; a.heads = heads; a.sq = rows; a.skv = rows;
+  a.scale_log2 = scale * 1.4426950408889634f;
+  a.ldo = ldo; a.out = out;
+  a.n_split = n_split; a.part_o = part_o; a.part_lse = part_lse;
+  a.seg_off = seg_off; a.n_seg = n_seg;
+  return check(f3r::launch_attention_segments(tq, tkv, a, static_cast<int>(max_tiles), static_cast<cudaStream_t>(stream)),
+               what);
+}
+
 int f3r_attention_merge(const float* part_o, const float* part_lse, int32_t n_parts, void* out, int32_t ldo,
                         int32_t batch, int32_t heads, int32_t sq, void* stream) {
   if (!part_o || !part_lse || !out || n_parts < 1) return fail("f3r_attention_merge: bad arguments");

@@ -110,10 +110,17 @@ struct AttnArgs {
   int part_base;
   float* part_o;              // fp32 [slots, batch*sq, heads*64]
   float* part_lse;            // fp32 [slots, batch, heads, sq]
+  // segment mode (launch_attention_segments): batch = 1, sq = skv = all rows; segment s is rows
+  // [seg_off[s], seg_off[s+1]) and attends to its own rows only
+  const int* seg_off;         // device int32 [n_seg + 1]
+  int n_seg;
 };
 cudaError_t launch_attention_merge(const float* part_o, const float* part_lse, int n_parts, int batch, int heads, int sq,
                                    void* out, int ldo, cudaStream_t stream);
 cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, cudaStream_t stream);
+// segment mode: grid of heads * n_split * max_tiles CTAs, max_tiles >= the total query tiles of all segments
+cudaError_t launch_attention_segments(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, int max_tiles,
+                                      cudaStream_t stream);
 
 // parity mode (attention_x3.cu): hi/lo-split bf16 operands, fp32 out (AttnArgs.out is float*)
 cudaError_t launch_attention_x3(const CUtensorMap& tq3, const CUtensorMap& tk3, const CUtensorMap& tv2,

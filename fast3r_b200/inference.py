@@ -185,11 +185,8 @@ class _precision_scope:
             self.model.precision = self.prev
 
 
-def loss_of_one_batch(batch, model, criterion, device, precision, symmetrize_batch=False, use_amp=False, ret=None,
-                      profiling=False):
-    """fast3r/dust3r/inference_multiview.py:22-67 (H2D of the view tensors, precision selection, model call, optional
-    criterion)."""
-    device = torch.device(device)
+def _upload(batch, model, device):
+    """H2D of the view tensors of one collated sample, in place."""
     sharded = getattr(model, "sp_group", None) is not None  # sequence parallel: the model uploads only its own views
     for view in batch:
         for name in _MOVE_KEYS:
@@ -199,6 +196,26 @@ def loss_of_one_batch(batch, model, criterion, device, precision, symmetrize_bat
             view[name] = src.to(device, non_blocking=True)
             if _KEEP_HOST_REFS and src.device.type == "cpu" and device.type != "cpu":
                 view.setdefault("_host_copy", {})[name] = src  # lets inference() hand the same host tensor back
+
+
+def _views_to_cpu(views):
+    """The views of a result on the host.  The reference copies the (just uploaded) inputs back to the host (to_cpu(res),
+    inference_multiview.py:92); the bytes are identical to the caller's host tensors, so those are returned instead of a
+    second PCIe transfer.  NOTE: the returned views' "img" therefore ALIASES the caller's input tensor (the reference
+    returns a copy)."""
+    views_cpu = []
+    for view in views:
+        host = view.pop("_host_copy", {})
+        views_cpu.append({k: (host[k] if k in host else to_cpu(v)) for k, v in view.items()})
+    return views_cpu
+
+
+def loss_of_one_batch(batch, model, criterion, device, precision, symmetrize_batch=False, use_amp=False, ret=None,
+                      profiling=False):
+    """fast3r/dust3r/inference_multiview.py:22-67 (H2D of the view tensors, precision selection, model call, optional
+    criterion)."""
+    device = torch.device(device)
+    _upload(batch, model, device)
     views = batch
     with _precision_scope(model, precision):
         if profiling:
@@ -236,16 +253,47 @@ def inference(multiple_views_in_one_sample, model, device, dtype, verbose=True, 
     profiling_info = None
     if profiling and "profiling_info" in res:
         profiling_info = res.pop("profiling_info")
-    # views: the reference copies the (just uploaded) inputs back to the host (to_cpu(res), :92); the bytes are
-    # identical to the caller's host tensors, so those are returned instead of a second PCIe transfer.  NOTE: the
-    # returned result["views"][i]["img"] therefore ALIASES the caller's input tensor (the reference returns a copy).
-    views_cpu = []
-    for view in res["views"]:
-        host = view.pop("_host_copy", {})
-        views_cpu.append({k: (host[k] if k in host else to_cpu(v)) for k, v in view.items()})
-    res = dict(views=views_cpu, preds=_preds_to_cpu(res["preds"], prefilled), loss=to_cpu(res["loss"]))
+    res = dict(views=_views_to_cpu(res["views"]), preds=_preds_to_cpu(res["preds"], prefilled), loss=to_cpu(res["loss"]))
     result.append(res)
     result = collate_with_cat(result, lists=multiple_shapes)
     if profiling and profiling_info is not None:
+        return result, profiling_info
+    return result
+
+
+@torch.no_grad()
+def inference_many(samples, model, device, dtype, verbose=True, profiling=False):
+    """Several scenes in one model call (Fast3R.forward_many).  ``samples``: a list of view lists, one per scene.
+    Returns a list whose element i has the structure of ``inference(samples[i], model, device, dtype)``: ``views``,
+    ``preds`` and ``loss=None``, on the host; with ``profiling``, (that list, one profiling_info for the whole call).
+    The image ids are drawn per scene in scene order, as a loop of inference() calls draws them."""
+    if verbose:
+        print(f">> Inference with model on {len(samples)} samples, {sum(len(s) for s in samples)} images")
+    global _KEEP_HOST_REFS
+    _KEEP_HOST_REFS = True
+    dev = torch.device(device)
+    sink = _HostSink(dev) if (dev.type == "cuda" and hasattr(model, "_host_sink")) else None
+    batches = [collate_with_cat([tuple(views)]) for views in samples]
+    try:
+        if sink is not None:
+            model._host_sink = sink
+        for batch in batches:
+            _upload(batch, model, dev)
+        with _precision_scope(model, dtype):
+            out = model.forward_many(batches, profiling=profiling)
+    finally:
+        _KEEP_HOST_REFS = False
+        if sink is not None:
+            model._host_sink = None
+    preds, profiling_info = out if profiling else (out, None)
+    prefilled = sink.finish() if sink is not None else None
+    # one D2H pass over all samples: the predictions of a shape group share their device buffers across samples
+    flat = _preds_to_cpu([p for sample in preds for p in sample], prefilled)
+    result, k = [], 0
+    for views, batch, sample in zip(samples, batches, preds):
+        res = dict(views=_views_to_cpu(batch), preds=flat[k:k + len(sample)], loss=None)
+        k += len(sample)
+        result.append(collate_with_cat([res], lists=not check_if_same_size(views)))
+    if profiling:
         return result, profiling_info
     return result

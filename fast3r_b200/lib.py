@@ -62,6 +62,7 @@ _API = {
     "f3r_attention": (C.c_int, [_P, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _F32, _P]),
     "f3r_attention_partial": (C.c_int, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _P, _P, _I32, _I32, _I32, _I32,
                                         _F32, _P]),
+    "f3r_attention_segments": (C.c_int, [_P, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _F32, _I32, _P, _P, _P]),
     "f3r_attention_merge": (C.c_int, [_P, _P, _I32, _P, _I32, _I32, _I32, _I32, _P]),
     "f3r_layernorm": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _F32, _P]),
     "f3r_im2col_patch": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _P]),

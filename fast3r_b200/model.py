@@ -24,6 +24,7 @@ import torch.nn as nn
 
 from . import lib as L
 from . import ops
+from .ops import Segments
 
 try:  # same hub integration as the reference (fast3r/models/fast3r.py:45-49): from_pretrained / save_pretrained
     from huggingface_hub import PyTorchModelHubMixin as _HubMixin
@@ -453,7 +454,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
 
     # ---- one transformer block (fast3r/croco/models/blocks.py:135-194, 236-239)
     @staticmethod
-    def _block(x, w: _BlockW, ws, *, batch, seq, heads, eps, scale, rope=None, kv_exchange=None):
+    def _block(x, w: _BlockW, ws, *, batch, seq, heads, eps, scale, rope=None, kv_exchange=None, segments=None):
         M, D = x.shape
         h, q, kv, att, hid = ws["h"][:M], ws["q"][:M], ws["kv"][:M], ws["att"][:M], ws["hid"][:M]
         ops.layernorm(x, w.n1w, w.n1b, eps, h)
@@ -463,7 +464,13 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
                      rope_sin=rope["sin"])
         else:
             w.linear(h, w.qkv_w, w.qkv_b, out0=q, ldo=D, split_col=D, out0b=kv, ldo_b=2 * D)
-        if kv_exchange is None:
+        if segments is not None:  # several samples in one sequence (forward_many): each attends to its own tokens
+            if w.x3:  # parity path: one attention per segment
+                for a, b in zip(segments.offsets, segments.offsets[1:]):
+                    ops.attention_x3(q[a:b], kv[a:b], att[a:b], batch=1, heads=heads, sq=b - a, skv=b - a, scale=scale)
+            else:
+                ops.attention_segments(q, kv, att, segments, heads=heads, scale=scale)
+        elif kv_exchange is None:
             (ops.attention_x3 if w.x3 else ops.attention)(q, kv, att, batch=batch, heads=heads, sq=seq, skv=seq,
                                                           scale=scale)
         else:  # sequence parallel: exchange K|V with the other ranks and attend to all keys (parallel.KVExchange)
@@ -507,10 +514,11 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
 
     # ---- fusion decoder (fast3r/models/fast3r.py:768-808)
     def _decode(self, feats_bnp: torch.Tensor, ids: torch.Tensor, B: int, seq: int, tok_per_img: int, P_: _ModelW,
-                kv_exchange=None):
+                kv_exchange=None, segments=None):
         """feats_bnp: (B*seq, D) tokens in (b, view, patch) order.  ids: image-index table rows, a (B, views) tensor
         with one row per view of tok_per_img tokens, or with tok_per_img=0 a flat (B*seq,) tensor with one row per
-        token (views of different resolutions)."""
+        token (views of different resolutions).  segments (ops.Segments, B = 1): the sequence holds several samples,
+        each attending to its own tokens only."""
         dec = self.decoder
         D = dec.embed_dim
         M = feats_bnp.shape[0]
@@ -533,7 +541,8 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
                 slot = kv_exchange.kv_workspace(ws["kv"].dtype, dev)
                 if slot is not None:
                     ws["kv"] = slot  # the QKV GEMM writes K|V straight into this rank's exchange slot of this layer
-            self._block(x, w, ws, batch=B, seq=seq, heads=dec.num_heads, eps=1e-5, scale=scale, kv_exchange=kv_exchange)
+            self._block(x, w, ws, batch=B, seq=seq, heads=dec.num_heads, eps=1e-5, scale=scale, kv_exchange=kv_exchange,
+                        segments=segments)
             self._tap(f"dec_block{i}", x)
             if (i + 1) in hooks:
                 if P_.x3:
@@ -691,22 +700,25 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         return flags
 
     # ---- forward (fast3r/models/fast3r.py:302-497)
-    def forward(self, views, profiling=False):
+    def _check_forward(self):
         if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError(
                 "fast3r_b200.Fast3R has no backward kernels (training step, SURVEY a13 / config 5, is not built): "
                 "call it under torch.no_grad() for a forward-only pass, or use model.eval()")
         if self.precision not in PRECISIONS:
             raise ValueError(f"precision must be one of {PRECISIONS}, got {self.precision!r}")
+
+    def forward(self, views, profiling=False):
+        self._check_forward()
         with torch.no_grad():
             return self._forward(views, profiling)
 
-    def _forward(self, views, profiling=False):
-        # (decorated with no_grad: the CUDA path has no backward kernels yet.  Training-mode FORWARD semantics - attention
-        # scale 1/8, fast3r/croco/models/blocks.py:151-154 - are honoured and tested; optimisation steps are not.)
-        profiling_info = {} if profiling else None
-        t_start = time.time()
-        N = len(views)
+    def _landscape(self, views):
+        """(batch size, images in the geometry the model runs them in, portrait flag per view) of one sample's views.
+        Portrait views (ManyAR_PatchEmbed + landscape_only heads) are recognised when all views share one stored shape.
+        They are un-transposed (a strided view of the same pixels) and run in their true geometry - patch grid, RoPE
+        positions and DPT head at (W, H); their predictions are transposed back to the landscape storage layout after
+        the heads, exactly what ManyAR_PatchEmbed + transpose_to_landscape.wrapper_yes compute."""
         B, _, H, W = views[0]["img"].shape
         ps = self.encoder.patch_size
         for v in views:
@@ -715,18 +727,143 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
                 raise ValueError("all views must have the same batch size")
             if h % ps or w % ps:
                 raise AssertionError(f"Input image size ({h}x{w}) is not a multiple of patch size ({ps}).")
-        # Portrait views (ManyAR_PatchEmbed + landscape_only heads) are recognised when all views share one stored
-        # shape.  They are un-transposed (a strided view of the same pixels) and run in their true geometry - patch grid,
-        # RoPE positions and DPT head at (W, H); their predictions are transposed back to the landscape storage layout
-        # below, exactly what ManyAR_PatchEmbed + transpose_to_landscape.wrapper_yes compute.
         same_shape = all(v["img"].shape == views[0]["img"].shape for v in views)
-        portrait = self._portrait_flags(views, H, W) if same_shape else [False] * N
+        portrait = self._portrait_flags(views, H, W) if same_shape else [False] * len(views)
         imgs = [v["img"].swapaxes(-1, -2) if p else v["img"] for v, p in zip(views, portrait)]
-        # Views of different resolutions (fast3r/models/fast3r.py:276-294, 364-376, 407-428): the reference encodes them
-        # and runs the heads view by view; here views are grouped by shape (same arithmetic per view, batched per group).
+        return B, imgs, portrait
+
+    @staticmethod
+    def _shape_groups(imgs) -> Dict[tuple, List[int]]:
+        """Views of different resolutions (fast3r/models/fast3r.py:276-294, 364-376, 407-428): the reference encodes them
+        and runs the heads view by view; here views are grouped by shape (same arithmetic per view, batched per group)."""
         groups: Dict[tuple, List[int]] = {}
         for i, im in enumerate(imgs):
             groups.setdefault(tuple(im.shape[-2:]), []).append(i)
+        return groups
+
+    def _encode_groups(self, imgs, groups, device, P_: _ModelW, keep=lambda i: True):
+        """Per shape group: ((H, W), its kept views, their encoder tokens in (view, b, patch) order, P, gh, gw)."""
+        enc = []
+        for shape, idxs in groups.items():
+            idxs = [i for i in idxs if keep(i)]
+            if not idxs:  # no view of this resolution on this rank
+                continue
+            x = torch.cat([imgs[i].to(device, non_blocking=True) for i in idxs], dim=0).to(dtype=F32).contiguous()
+            enc.append((shape, idxs) + self._encode(x, P_))
+        return enc
+
+    def _heads(self, enc, hooked, B, P_: _ModelW, device, results):
+        """The DPT heads of every shape group; view i's predictions go into results[i]."""
+        for ((H, W), idxs, _, P, gh, gw), hk in zip(enc, hooked):
+            outs = self._run_heads(hk, len(idxs) * B, P, gh, gw, H, W, P_, device)
+            for k, i in enumerate(idxs):
+                self._fill_result(results[i], outs, k, B)
+
+    @staticmethod
+    def _to_landscape(results, portrait):
+        for r, p in zip(results, portrait):
+            if p:
+                for k in list(r):
+                    r[k] = r[k].swapaxes(1, 2)
+
+    def _pack_tokens(self, enc, ids, off, t0, seq, B, P_: _ModelW, device):
+        """Decoder input with one image-index row per token, one index_copy / index_select per shape group instead of
+        per-view slices: each of the B sequences holds its views' tokens in (view, patch) order, view i at rows
+        [off[i] - t0, off[i] - t0 + P).  ids: (B, views) image ids.  Returns the (B*seq, D) tokens, their (B*seq,) ids,
+        and per group the map of a decoder output back to the group's (view, b, patch) order, the head input order."""
+        feats_bnp = torch.empty(B * seq, self.encoder.embed_dim, dtype=P_.adt, device=device)
+        tok_ids = torch.empty(B, seq, dtype=torch.int32)
+        to_heads = []
+        for _, idxs, feats, P, _, _ in enc:
+            base = torch.tensor([off[i] - t0 for i in idxs], dtype=torch.long)  # (n_g,)
+            r = (base[:, None, None] + torch.arange(B, dtype=torch.long)[None, :, None] * seq
+                 + torch.arange(P, dtype=torch.long)[None, None, :]).reshape(-1).to(device)  # (n_g, B, P) order
+            feats_bnp.index_copy_(0, r, feats)
+            for i in idxs:
+                tok_ids[:, off[i] - t0: off[i] - t0 + P] = ids[:, i:i + 1].to(torch.int32)
+            to_heads.append(lambda t, r=r: t.index_select(0, r))
+        return feats_bnp, tok_ids.reshape(-1), to_heads
+
+    def forward_many(self, samples, profiling=False):
+        """Several scenes in one forward.  ``samples``: a list of view lists, each of batch size 1 (what inference()
+        collates); returns one preds list per sample, each what ``forward(sample)`` returns (with ``profiling``, one
+        ``profiling_info`` for the whole call).  The encoder and the DPT heads batch the views of all samples by shape;
+        the decoder runs one sequence of all samples' tokens, sample after sample, whose fusion attention is block-
+        diagonal (ops.attention_segments): each sample's tokens attend to that sample's tokens only.  The image ids are
+        drawn per sample, in sample order, so the global torch RNG advances as for forward on each sample in turn.
+        Per sample, the result equals forward(sample) up to the order of fp32 sums: GEMM plans depend on the row count,
+        which packing changes.  forward_many([sample]) is bit-identical to forward(sample)."""
+        self._check_forward()
+        with torch.no_grad():
+            return self._forward_many(samples, profiling)
+
+    def _forward_many(self, samples, profiling=False):
+        if self.sp_group is not None:
+            raise NotImplementedError("forward_many does not run on a sequence-parallel (sharded) model; call forward "
+                                      "per sample")
+        if len(samples) == 0:
+            raise ValueError("forward_many: empty sample list")
+        profiling_info = {} if profiling else None
+        t_start = time.time()
+        flat_imgs, portraits = [], []  # all views of all samples, sample after sample
+        for s, views in enumerate(samples):
+            if len(views) == 0:
+                raise ValueError(f"forward_many: sample {s} has no views")
+            B, imgs, portrait = self._landscape(views)
+            if B != 1:
+                raise ValueError(f"forward_many packs samples of batch size 1 (sample {s} has {B}); call forward for it")
+            flat_imgs += imgs
+            portraits.append(portrait)
+        device = samples[0][0]["img"].device
+        P_ = self._pack(device)
+        ps = self.encoder.patch_size
+        enc = self._encode_groups(flat_imgs, self._shape_groups(flat_imgs), device, P_)
+        if profiling:
+            _sync(device)
+            profiling_info["encode_images_time"] = time.time() - t_start
+        t1 = time.time()
+        ids = torch.cat([self.decoder.draw_image_ids(1, len(views), rank_offset=self.image_id_rank_offset)
+                         for views in samples], dim=1)  # (1, all views)
+        if profiling:
+            profiling_info["pos_emb_time"] = time.time() - t1
+            _sync(device)
+        t2 = time.time()
+        off = list(accumulate([(im.shape[-2] // ps) * (im.shape[-1] // ps) for im in flat_imgs], initial=0))
+        first = list(accumulate([len(views) for views in samples], initial=0))  # first view of each sample
+        segments = Segments([off[i] for i in first], device)
+        feats_bnp, tok_ids, to_heads = self._pack_tokens(enc, ids, off, 0, off[-1], 1, P_, device)
+        dec_out = self._decode(feats_bnp, tok_ids, 1, off[-1], 0, P_, segments=segments)
+        if profiling:
+            _sync(device)
+            profiling_info["decoder_time"] = time.time() - t2
+        t3 = time.time()
+        hooked = [[feats] + [to_head(t) for t in dec_out] for (_, _, feats, _, _, _), to_head in zip(enc, to_heads)]
+        if profiling:
+            profiling_info["head_prepare_input_time"] = time.time() - t3
+        t4 = time.time()
+        flat_results = [{} for _ in flat_imgs]
+        self._heads(enc, hooked, 1, P_, device, flat_results)
+        results = [flat_results[a:b] for a, b in zip(first, first[1:])]
+        for r, portrait in zip(results, portraits):
+            self._to_landscape(r, portrait)
+        if profiling:
+            _sync(device)
+            t_end = time.time()
+            profiling_info["head_forward_time"] = t_end - t4
+            profiling_info["total_time"] = t_end - t_start
+            return results, profiling_info
+        return results
+
+    def _forward(self, views, profiling=False):
+        # (decorated with no_grad: the CUDA path has no backward kernels yet.  Training-mode FORWARD semantics - attention
+        # scale 1/8, fast3r/croco/models/blocks.py:151-154 - are honoured and tested; optimisation steps are not.)
+        profiling_info = {} if profiling else None
+        t_start = time.time()
+        N = len(views)
+        B, imgs, portrait = self._landscape(views)
+        H, W = views[0]["img"].shape[-2:]
+        ps = self.encoder.patch_size
+        groups = self._shape_groups(imgs)
         sp = self.sp_group
         device = views[0]["img"].device
         if sp is not None and device.type != "cuda":
@@ -736,13 +873,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         off = list(accumulate(tokens, initial=0))  # first token of each view in a sample's sequence
         # sequence parallel: contiguous views per rank, balanced by token count (views of different resolutions)
         lo, hi = (0, N) if sp is None else sp.view_range(N, tokens)
-        enc = []  # per group: ((H, W), this rank's views, their encoder tokens in (view, b, patch) order, P, gh, gw)
-        for shape, idxs in groups.items():
-            idxs = [i for i in idxs if lo <= i < hi]
-            if not idxs:  # no view of this resolution on this rank
-                continue
-            x = torch.cat([imgs[i].to(device, non_blocking=True) for i in idxs], dim=0).to(dtype=F32).contiguous()
-            enc.append((shape, idxs) + self._encode(x, P_))
+        enc = self._encode_groups(imgs, groups, device, P_, keep=lambda i: lo <= i < hi)
         if profiling:
             _sync(device)
             profiling_info["encode_images_time"] = time.time() - t_start
@@ -768,21 +899,10 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
                 n = len(idxs)
                 swap = lambda t, a, b: t.view(a, b, P, -1).permute(1, 0, 2, 3).contiguous().view(a * b * P, -1)  # noqa: E731
                 feats_bnp, to_heads = swap(feats, n, B), [lambda t: swap(t, B, n)]
-        else:  # one image-index row per token; one index_copy / index_select per group instead of per-view slices
+        else:
             t0 = off[lo]  # this rank's tokens are [off[lo], off[hi]) of each sample's sequence
             seq, tok_per_img = off[hi] - t0, 0
-            feats_bnp = torch.empty(B * seq, self.encoder.embed_dim, dtype=P_.adt, device=device)
-            tok_ids = torch.empty(B, seq, dtype=torch.int32)
-            to_heads = []
-            for _, idxs, feats, P, _, _ in enc:
-                base = torch.tensor([off[i] - t0 for i in idxs], dtype=torch.long)  # (n_g,)
-                r = (base[:, None, None] + torch.arange(B, dtype=torch.long)[None, :, None] * seq
-                     + torch.arange(P, dtype=torch.long)[None, None, :]).reshape(-1).to(device)  # (n_g, B, P) order
-                feats_bnp.index_copy_(0, r, feats)
-                for i in idxs:
-                    tok_ids[:, off[i] - t0: off[i] - t0 + P] = ids[:, i:i + 1].to(torch.int32)
-                to_heads.append(lambda t, r=r: t.index_select(0, r))
-            ids = tok_ids.reshape(-1)
+            feats_bnp, ids, to_heads = self._pack_tokens(enc, ids, off, t0, seq, B, P_, device)
         kvx = None
         if sp is not None:
             kvx = sp.make_kv_exchange(B, seq, self.decoder.embed_dim, rows=[off[b] - off[a] for a, b in sp.ranges],
@@ -797,14 +917,8 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
             profiling_info["head_prepare_input_time"] = time.time() - t3
         t4 = time.time()
         final_results = [{} for _ in range(N)]
-        for ((H, W), idxs, _, P, gh, gw), hk in zip(enc, hooked):
-            outs = self._run_heads(hk, len(idxs) * B, P, gh, gw, H, W, P_, device)
-            for k, i in enumerate(idxs):
-                self._fill_result(final_results[i], outs, k, B)
-        for r, p in zip(final_results, portrait):
-            if p:
-                for k in list(r):
-                    r[k] = r[k].swapaxes(1, 2)
+        self._heads(enc, hooked, B, P_, device, final_results)
+        self._to_landscape(final_results, portrait)
         if sp is not None and sp.gather_preds:
             final_results = sp.gather_results(final_results, N, B, H, W, device,
                                               shapes=[v["img"].shape[-2:] for v in views])

@@ -207,6 +207,55 @@ def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: in
         timer.append((batch, heads, sq, skv, e0, e1))
 
 
+class Segments:
+    """Segment boundaries of a packed sequence, for attention_segments: the host offsets (they size the launch and pick
+    the key split) and their int32 device copy, uploaded once for every call that shares them."""
+
+    def __init__(self, offsets, device):
+        self.offsets = [int(v) for v in offsets]
+        if len(self.offsets) < 2 or self.offsets[0] != 0 or any(b < a for a, b in zip(self.offsets, self.offsets[1:])):
+            raise ValueError(f"segment offsets must start at 0 and not decrease, got {self.offsets}")
+        self.device_offsets = torch.tensor(self.offsets, dtype=torch.int32).to(device)
+
+    @property
+    def rows(self) -> int:
+        return self.offsets[-1]
+
+    def lengths(self):
+        return [b - a for a, b in zip(self.offsets, self.offsets[1:])]
+
+
+def attention_segments(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, seg_off, *, heads: int, scale: float,
+                       kv_split: Optional[int] = None):
+    """Block-diagonal attention in one launch (f3r_attention_segments): q (rows, ldq), kv (rows, ldkv) [K | V] and out
+    (rows, ldo), bf16; the rows [seg_off[s], seg_off[s+1]) attend to those rows only, each segment exactly as
+    attention(batch=1) over it alone with the same key split.  seg_off: a Segments, or the offsets as a host sequence.
+    kv_split: key slices per segment (a segment with fewer key blocks uses one per block); None picks it with
+    pick_kv_split over all the launch's query tiles."""
+    _chk(q, BF16, "q"); _chk(kv, BF16, "kv"); _chk(out, BF16, "out")
+    if not isinstance(seg_off, Segments):
+        seg_off = Segments(seg_off, q.device)
+    rows = seg_off.rows
+    ldq, ldkv, ldo = q.shape[-1], kv.shape[-1], out.shape[-1]
+    assert q.numel() == rows * ldq and kv.numel() == rows * ldkv and out.numel() == rows * ldo
+    lens = seg_off.lengths()
+    key_blocks = max(-(-n // 128) for n in lens)
+    if kv_split is None:
+        units = sum(attention_units(1, heads, n) for n in lens)
+        kv_split = pick_kv_split(units, key_blocks)
+    ns = max(1, min(kv_split, key_blocks))
+    n_seg, dev_off = len(lens), _ptr(seg_off.device_offsets)
+    if ns > 1:
+        part_o = torch.empty(ns, rows, heads * 64, dtype=F32, device=q.device)
+        part_lse = torch.empty(ns, heads, rows, dtype=F32, device=q.device)
+        _call("f3r_attention_segments", q, _ptr(q), ldq, _ptr(kv), ldkv, None, 0, dev_off, n_seg, rows, heads,
+              float(scale), ns, _ptr(part_o), _ptr(part_lse))
+        attention_merge(part_o, part_lse, ns, out, batch=1, heads=heads, sq=rows)
+    else:
+        _call("f3r_attention_segments", q, _ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, dev_off, n_seg, rows, heads,
+              float(scale), 1, None, None)
+
+
 def attention_x3(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: int, heads: int, sq: int, skv: int,
                  scale: float, lse: Optional[torch.Tensor] = None):
     """Parity-mode attention: q (batch*sq, ldq), kv (batch*skv, ldkv) [K | V], out (batch*sq, ldo), all fp32."""

@@ -100,6 +100,18 @@ int f3r_attention(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void
 int f3r_attention_partial(const void* q, int32_t ldq, const void* kv, int32_t ldkv, int32_t kv_rows_total,
                           int32_t kv_row0, int32_t skv, int32_t n_split, float* part_o, float* part_lse,
                           int32_t part_base, int32_t batch, int32_t heads, int32_t sq, float scale, void* stream);
+/* Block-diagonal form of f3r_attention, for several independent sequences packed into one (Fast3R.forward_many): q bf16
+ * [rows, ldq], kv bf16 [rows, ldkv] ([K | V] as in f3r_attention), out bf16 [rows, ldo].  seg_off: device int32
+ * [n_seg + 1], non-decreasing, seg_off[0] = 0 and seg_off[n_seg] = rows; the rows [seg_off[s], seg_off[s+1]) of
+ * segment s attend to those rows only, and every row gets exactly what f3r_attention (batch 1) over its segment alone
+ * computes.  Rows of other segments never reach a segment's result, NaN or Inf included.  One launch for all segments.
+ * n_split > 1: key slices as in f3r_attention_partial; slice s writes slot s of part_o (fp32 [n_split, rows, heads*64])
+ * and part_lse (fp32 [n_split, heads, rows]) and out is not written: f3r_attention_merge (batch 1, sq = rows,
+ * n_parts = n_split) gives the result.  A segment of fewer than n_split key blocks uses one slice per block and writes
+ * neutral partials (0, -inf) into its other slots, so it matches f3r_attention_partial with that many slices. */
+int f3r_attention_segments(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo,
+                           const int32_t* seg_off, int32_t n_seg, int32_t rows, int32_t heads, float scale,
+                           int32_t n_split, float* part_o, float* part_lse, void* stream);
 int f3r_attention_merge(const float* part_o, const float* part_lse, int32_t n_parts, void* out, int32_t ldo,
                         int32_t batch, int32_t heads, int32_t sq, void* stream);
 
