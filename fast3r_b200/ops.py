@@ -182,7 +182,12 @@ def attention_merge(part_o: torch.Tensor, part_lse: torch.Tensor, n_parts: int, 
 def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: int, heads: int, sq: int, skv: int,
               scale: float, lse: Optional[torch.Tensor] = None, kv_split: Optional[int] = None):
     """q (batch*sq, ldq) bf16, kv (batch*skv, ldkv) bf16 [K | V], out (batch*sq, ldo) bf16.  When the launch would
-    leave SMs idle (few query tiles), the keys are cut into slices (more CTAs) and merged (pick_kv_split)."""
+    leave SMs idle (few query tiles), the keys are cut into slices (more CTAs) and merged (pick_kv_split).  lse (batch,
+    heads, sq) fp32 receives the log-sum-exp of the scaled scores; it is written by the one-slice kernel only, so lse with
+    kv_split > 1 is refused."""
+    if lse is not None and kv_split is not None and kv_split > 1:
+        raise ValueError("ops.attention: lse is only written without key slices (kv_split > 1 merges partials that "
+                         "carry no log-sum-exp output)")
     _chk(q, BF16, "q"); _chk(kv, BF16, "kv"); _chk(out, BF16, "out")
     ldq, ldkv, ldo = q.shape[-1], kv.shape[-1], out.shape[-1]
     assert q.numel() == batch * sq * ldq and kv.numel() == batch * skv * ldkv and out.numel() == batch * sq * ldo

@@ -24,7 +24,6 @@ kernel's fp32 norm and exp); with d = |o_xyz| and g(d) = expm1(d) / d,
 The relative L2 error over each output is checked as well: the per-element bound catches a wrong element or tile, the
 L2 check a systematic drift that stays inside the bound.  Every element outside the region a call may write (canaries
 before and after each output, the columns beyond n for ldo > n, the other side of a column split) must keep its value."""
-import math
 import os
 
 import pytest
@@ -32,22 +31,11 @@ import torch
 import torch.nn.functional as F
 
 from tests import gemm_plans as GP
+from tests.canaries import buffer as _buffer, check_elements, untouched as _untouched, region as _region
 
 pytestmark = pytest.mark.gpu
 
-PAD = 64  # canary elements before and after every output (keeps 16-byte alignment)
-SENTINEL = -1234.5
 REL_L2 = {"bf16": 6e-3, "f32": 3e-5, "final": 2e-3}
-
-
-def _buffer(shape, dtype, fill=None):
-    """(full flat buffer, contiguous view of `shape` in its middle); the canaries hold SENTINEL."""
-    n = math.prod(shape)
-    buf = torch.full((n + 2 * PAD,), SENTINEL, dtype=dtype, device="cuda")
-    view = buf[PAD:PAD + n].view(shape)
-    if fill is not None:
-        view.copy_(fill)
-    return buf, view
 
 
 def _unfold(a, taps):
@@ -67,31 +55,10 @@ def _rope_tables(max_pos=256, base=100.0):
 
 
 def _check(name, out, ref, bound, kind):
+    check_elements(name, out, ref, bound)
     out = out.double()
-    err = (out - ref).abs()
-    bad = ~(err <= bound)  # NaN counts as bad
-    if bool(bad.any()):
-        idx = bad.nonzero()[:5].tolist()
-        worst = float((err / bound.clamp_min(1e-300)).nan_to_num(float("inf")).max())
-        raise AssertionError(f"{name}: {int(bad.sum())} of {out.numel()} elements outside the bound (worst {worst:.3g}x "
-                             f"the bound); first at {idx}: out {[float(out[tuple(i)]) for i in idx]} "
-                             f"ref {[float(ref[tuple(i)]) for i in idx]}")
     rel = float((out - ref).norm() / ref.norm().clamp_min(1e-30))
     assert rel <= REL_L2[kind], f"{name}: relative L2 error {rel:.3g} > {REL_L2[kind]}"
-
-
-def _untouched(name, buf, before, written):
-    """Elements of buf outside `written` (a bool mask of buf's shape) still hold their old bits."""
-    keep = ~written
-    a, b = buf[keep], before[keep]
-    same = (a == b) | (a.isnan() & b.isnan())
-    assert bool(same.all()), f"{name}: {int((~same).sum())} elements outside the written region changed"
-
-
-def _region(buf_len, rows, ld, cols, offset=PAD):
-    m = torch.zeros(buf_len, dtype=torch.bool, device="cuda")
-    m[offset:offset + rows * ld].view(rows, ld)[:, :cols] = True
-    return m
 
 
 def run_case(c, seed):
