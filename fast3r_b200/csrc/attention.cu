@@ -19,7 +19,9 @@
 // with two consumer warpgroups.
 // The arithmetic (ex2 inputs, order of the l and O updates, lazy-rescale decisions) is that of a loop that finishes one
 // key block before it starts the next, so the overlap does not change a bit of the result.
-// Segment mode (attention_kernel<true>, f3r_attention_segments): block-diagonal attention over the segments of one packed
+// fp16 (attention_kernel<..., __half>, the f3r_attention*_f16 entry points): Q, K, V, P and O are fp16 instead of bf16,
+// with the same tiles, pipeline and fp32 softmax; P is packed with cvt.rn.f16x2.f32.
+// Segment mode (attention_kernel<true, T>, f3r_attention_segments): block-diagonal attention over the segments of one packed
 // sequence, each segment with the arithmetic of a launch over it alone.
 #include "common.cuh"
 #include "f3r_kernels.h"
@@ -42,18 +44,20 @@ F3R_DEVICE float ex2_approx(float x) {
 }
 
 // S (64 rows x 128 keys of this warpgroup) = Q K^T, four k16 steps; committed as one wgmma group
+template <typename T>
 F3R_DEVICE void att_issue_s(float (&s)[64], uint64_t qd, const uint8_t* smem_k_stage) {
   const uint64_t kd = make_smem_desc_sw128(smem_u32(smem_k_stage));
 #pragma unroll
-  for (int k = 0; k < 4; ++k) wgmma_ss_n128<0>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
+  for (int k = 0; k < 4; ++k) wgmma_ss_n128<0, T>(s, qd + 2 * k, kd + 2 * k, k > 0 ? 1u : 0u);
   wgmma_commit();
 }
 
 // O += P V, eight k16 steps of 16 keys (16 smem rows = 2048 B of V); committed as one wgmma group
+template <typename T>
 F3R_DEVICE void att_issue_pv(float (&o)[32], const uint32_t (&pa)[8][4], const uint8_t* smem_v_stage) {
   const uint64_t vd = make_smem_desc_sw128(smem_u32(smem_v_stage));
 #pragma unroll
-  for (int kk = 0; kk < 8; ++kk) wgmma_rs_n64<1>(o, pa[kk], vd + 128 * kk, 1u);
+  for (int kk = 0; kk < 8; ++kk) wgmma_rs_n64<1, T>(o, pa[kk], vd + 128 * kk, 1u);
   wgmma_commit();
 }
 
@@ -98,7 +102,9 @@ F3R_DEVICE void att_softmax(float (&s)[64], int valid, int cq, float sl2, float 
   }
 }
 
-// After the last PV that read pa has landed: O *= alpha where the softmax moved the reference, then P -> bf16 A fragments
+// After the last PV that read pa has landed: O *= alpha where the softmax moved the reference, then P -> 16-bit A
+// fragments
+template <typename T>
 F3R_DEVICE void att_rescale_pack(float (&o)[32], uint32_t (&pa)[8][4], const float (&s)[64], const bool (&resc)[2],
                                  const float (&alpha)[2]) {
 #pragma unroll
@@ -110,7 +116,7 @@ F3R_DEVICE void att_rescale_pack(float (&o)[32], uint32_t (&pa)[8][4], const flo
 #pragma unroll
   for (int kk = 0; kk < 8; ++kk)
 #pragma unroll
-    for (int r = 0; r < 4; ++r) pa[kk][r] = pack_bf16(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+    for (int r = 0; r < 4; ++r) pa[kk][r] = Half16<T>::pack(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
 }
 
 // Segment mode: finds the segment of work item `item`.  Items are numbered segment by segment, heads * n_split per query
@@ -149,7 +155,8 @@ F3R_DEVICE bool att_find_segment(const AttnArgs& p, int item, int& s0, int& len,
 // rows only, with key blocks that start at its first row, so its rows get exactly the arithmetic of a kSeg = false launch
 // over that segment alone.  A segment with fewer key blocks than p.n_split uses one slice per key block and fills the
 // slots of its other slices with neutral partials (O = 0, LSE = -inf: merge weight 0).
-template <bool kSeg>
+// T: the type of Q, K, V and O (__nv_bfloat16 or __half).
+template <bool kSeg, typename T>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_kv,
                  const __grid_constant__ AttnArgs p) {
@@ -260,7 +267,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
     float s[64];         // S of the block in softmax, then its exponentials until they are packed
-    uint32_t pa[8][4];   // P of the block whose PV is in flight (bf16 A fragments)
+    uint32_t pa[8][4];   // P of the block whose PV is in flight (16-bit A fragments)
     bool resc[2];        // O rescale decided by the latest softmax ...
     float alpha[2];      // ... and its factor
     const uint64_t qd = make_smem_desc_sw128(smem_u32(smem_q + cg * 64 * 128));
@@ -271,7 +278,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     // block 0: S_0 and its softmax
     mbar_wait(&k_full[0], 0);
     wgmma_fence();
-    att_issue_s(s, qd, smem_k);
+    att_issue_s<T>(s, qd, smem_k);
     wgmma_wait<0>();
     fence_regs(s);
     if (wg_tid == 0) mbar_arrive(&k_empty[0]);
@@ -288,10 +295,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       wgmma_wait<0>();  // PV_{j-1} has landed: O may be rescaled and the P registers rewritten
       fence_regs(o);
       if (j > 0 && wg_tid == 0) mbar_arrive(&v_empty[(j - 1) % ATT_STAGES]);
-      att_rescale_pack(o, pa, s, resc, alpha);
+      att_rescale_pack<T>(o, pa, s, resc, alpha);
       wgmma_fence();
-      att_issue_s(s, qd, smem_k + sk * ATT_TILE_BYTES);
-      att_issue_pv(o, pa, smem_v + sv * ATT_TILE_BYTES);
+      att_issue_s<T>(s, qd, smem_k + sk * ATT_TILE_BYTES);
+      att_issue_pv<T>(o, pa, smem_v + sv * ATT_TILE_BYTES);
       wgmma_wait<1>();  // S_{j+1} has landed (groups complete in order)
       fence_regs(s);
       if (wg_tid == 0) mbar_arrive(&k_empty[sk]);
@@ -317,9 +324,9 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       wgmma_wait<0>();
       fence_regs(o);
       if (nkv > 1 && wg_tid == 0) mbar_arrive(&v_empty[(nkv - 2) % ATT_STAGES]);
-      att_rescale_pack(o, pa, s, resc, alpha);
+      att_rescale_pack<T>(o, pa, s, resc, alpha);
       wgmma_fence();
-      att_issue_pv(o, pa, smem_v + sv * ATT_TILE_BYTES);
+      att_issue_pv<T>(o, pa, smem_v + sv * ATT_TILE_BYTES);
       wgmma_wait<0>();
       fence_regs(o);
       if (wg_tid == 0) mbar_arrive(&v_empty[sv]);
@@ -348,33 +355,37 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           *reinterpret_cast<float2*>(dstf + 8 * jn) = make_float2(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv);
         if ((lane & 3) == 0) p.part_lse[(slot * p.batch * p.heads + static_cast<size_t>(b) * p.heads + h) * p.sq + qs] = lse;
       } else {
-        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.out) + (static_cast<size_t>(b) * p.sq + qs) * p.ldo + h * 64 + cq;
+        T* dst = static_cast<T*>(p.out) + (static_cast<size_t>(b) * p.sq + qs) * p.ldo + h * 64 + cq;
 #pragma unroll
         for (int jn = 0; jn < 8; ++jn)
-          *reinterpret_cast<uint32_t*>(dst + 8 * jn) = pack_bf16(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv);
+          *reinterpret_cast<uint32_t*>(dst + 8 * jn) =
+              Half16<T>::pack(o[4 * jn + 2 * hh] * inv, o[4 * jn + 2 * hh + 1] * inv);
         if (p.lse != nullptr && (lane & 3) == 0) p.lse[(static_cast<size_t>(b) * p.heads + h) * p.sq + qs] = lse;
       }
     }
   }
 }
 
-cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, cudaStream_t stream) {
-  return launch(attention_kernel<false>, a.batch * a.heads * a.q_tiles * a.n_split, ATT_THREADS, ATT_SMEM_BYTES, stream,
-                true, tq, tkv, a);
+cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, int f16,
+                             cudaStream_t stream) {
+  return launch(f16 ? attention_kernel<false, __half> : attention_kernel<false, __nv_bfloat16>,
+                a.batch * a.heads * a.q_tiles * a.n_split, ATT_THREADS, ATT_SMEM_BYTES, stream, true, tq, tkv, a);
 }
 
 cudaError_t launch_attention_segments(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, int max_tiles,
-                                      cudaStream_t stream) {
-  return launch(attention_kernel<true>, a.heads * a.n_split * max_tiles, ATT_THREADS, ATT_SMEM_BYTES, stream, true, tq,
-                tkv, a);
+                                      int f16, cudaStream_t stream) {
+  return launch(f16 ? attention_kernel<true, __half> : attention_kernel<true, __nv_bfloat16>,
+                a.heads * a.n_split * max_tiles, ATT_THREADS, ATT_SMEM_BYTES, stream, true, tq, tkv, a);
 }
 
 // ---------------------------------------------------------------- merge of key-slice partials
 // out[row, h*64 + d] = sum_p w_p O_p[row, h, d] / sum_p w_p,  w_p = exp(lse_p - max_p lse_p): the exact softmax over the
-// union of the slices (each O_p is normalised over its own slice).  8 threads per (row, head), 8 columns each.
+// union of the slices (each O_p is normalised over its own slice).  8 threads per (row, head), 8 columns each.  T: the
+// type of out (__nv_bfloat16 or __half).
+template <typename T>
 __global__ void __launch_bounds__(256) attention_merge_kernel(const float* __restrict__ part_o,
                                                               const float* __restrict__ part_lse, int n_parts, int batch,
-                                                              int heads, int sq, __nv_bfloat16* __restrict__ out, int ldo) {
+                                                              int heads, int sq, T* __restrict__ out, int ldo) {
   pdl_wait();                // the partials come from the preceding attention launches
   pdl_launch_dependents();
   const size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
@@ -400,16 +411,21 @@ __global__ void __launch_bounds__(256) attention_merge_kernel(const float* __res
   }
   const float inv = 1.f / wsum;
   uint4 o;
-  o.x = pack_bf16(acc[0] * inv, acc[1] * inv); o.y = pack_bf16(acc[2] * inv, acc[3] * inv);
-  o.z = pack_bf16(acc[4] * inv, acc[5] * inv); o.w = pack_bf16(acc[6] * inv, acc[7] * inv);
+  using H = Half16<T>;
+  o.x = H::pack(acc[0] * inv, acc[1] * inv); o.y = H::pack(acc[2] * inv, acc[3] * inv);
+  o.z = H::pack(acc[4] * inv, acc[5] * inv); o.w = H::pack(acc[6] * inv, acc[7] * inv);
   *reinterpret_cast<uint4*>(out + m * ldo + h * 64 + g * 8) = o;
 }
 cudaError_t launch_attention_merge(const float* part_o, const float* part_lse, int n_parts, int batch, int heads, int sq,
-                                   void* out, int ldo, cudaStream_t stream) {
+                                   void* out, int ldo, int f16, cudaStream_t stream) {
   const size_t total = static_cast<size_t>(batch) * sq * heads * 8;
   if (total == 0) return cudaSuccess;
-  return launch(attention_merge_kernel, static_cast<unsigned>((total + 255) / 256), 256, 0, stream, true, part_o, part_lse,
-                n_parts, batch, heads, sq, static_cast<__nv_bfloat16*>(out), ldo);
+  const unsigned grid = static_cast<unsigned>((total + 255) / 256);
+  if (f16)
+    return launch(attention_merge_kernel<__half>, grid, 256, 0, stream, true, part_o, part_lse, n_parts, batch, heads, sq,
+                  static_cast<__half*>(out), ldo);
+  return launch(attention_merge_kernel<__nv_bfloat16>, grid, 256, 0, stream, true, part_o, part_lse, n_parts, batch,
+                heads, sq, static_cast<__nv_bfloat16*>(out), ldo);
 }
 
 }  // namespace f3r

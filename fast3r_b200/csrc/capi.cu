@@ -104,6 +104,7 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
     return fail("f3r_gemm: bad ROPE arguments");
   if (d->epi == F3R_EPI_IDXEMB && (!d->emb_table || !d->emb_ids || d->tok_per_img < 0))
     return fail("f3r_gemm: bad IDXEMB arguments");
+  if (d->f16 != 0 && d->f16 != 1) return fail("f3r_gemm: f16=%d must be 0 or 1", d->f16);
 
   static int dbg = -1, tma_pref = -1, ksplit_pref = -1;
   if (dbg < 0) { const char* e = getenv("F3R_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }
@@ -134,6 +135,8 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
   a.w4 = d->w4; a.b4 = d->b4; a.pts = d->pts; a.conf = d->conf;
   if (a.split_col && (a.split_col % 32 || !a.out0b)) return fail("f3r_gemm: bad column split");
 
+  // the 16-bit operands and outputs: bf16, or fp16 with d->f16
+  const CUtensorMapDataType t16 = d->f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   CUtensorMap ta, tb;
   {
     const uint64_t ld = static_cast<uint64_t>(d->a_ld) * 2;
@@ -141,14 +144,14 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
                               static_cast<uint64_t>(d->h), static_cast<uint64_t>(d->nb)};
     const uint64_t str[3] = {ld, ld * d->w, ld * d->w * d->h};
     const uint32_t box[4] = {64, static_cast<uint32_t>(a.bw), static_cast<uint32_t>(a.bh), 1};
-    if (make_tmap(&ta, d->a, 4, dims, str, box)) return 1;
+    if (make_tmap(&ta, d->a, 4, dims, str, box, t16)) return 1;
   }
   {
     const uint64_t dims[3] = {static_cast<uint64_t>(d->k), static_cast<uint64_t>(d->taps),
                               static_cast<uint64_t>(d->n)};
     const uint64_t str[2] = {static_cast<uint64_t>(d->k) * 2, static_cast<uint64_t>(d->k) * 2 * d->taps};
     const uint32_t box[3] = {64, 1, static_cast<uint32_t>(block_n)};
-    if (make_tmap(&tb, d->wt, 3, dims, str, box)) return 1;
+    if (make_tmap(&tb, d->wt, 3, dims, str, box, t16)) return 1;
   }
   // output tensor maps of the TMA epilogue (plan.tma_epi: plain stores, or the in-place fp32 residual reduce-add)
   CUtensorMap to0, to0b;
@@ -156,7 +159,7 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
   memset(&to0b, 0, sizeof(to0b));
   if (a.tma_epi) {
     const uint64_t es = d->out0_f32 ? 4 : 2;
-    const CUtensorMapDataType dt = d->out0_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+    const CUtensorMapDataType dt = d->out0_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : t16;
     const CUtensorMapSwizzle sw = d->out0_f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
     const uint32_t sbx = 1u << a.sbx_log2;
     const uint32_t box[4] = {32, sbx, 32 / sbx, 1};
@@ -176,14 +179,16 @@ int f3r_gemm(const f3r_gemm_desc* d, void* stream) {
       if (make_tmap(&to0b, d->out0b, 4, dims, str, box, dt, sw)) return 1;
     }
   }
-  return check(f3r::launch_gemm(block_n, ta, tb, to0, to0b, a, num_sms(), static_cast<cudaStream_t>(stream)),
+  return check(f3r::launch_gemm(block_n, d->f16, ta, tb, to0, to0b, a, num_sms(), static_cast<cudaStream_t>(stream)),
                "f3r_gemm");
 }
 
-static int attention_impl(const char* what, const void* q, int32_t ldq, const void* kv, int32_t ldkv,
+// f16: q, kv and out are fp16 (the *_f16 entry points) instead of bf16
+static int attention_impl(const char* what, int f16, const void* q, int32_t ldq, const void* kv, int32_t ldkv,
                           int32_t kv_rows_total, int32_t kv_row0, void* out, int32_t ldo, float* lse, float* part_o,
                           float* part_lse, int32_t part_base, int32_t n_split, int32_t batch, int32_t heads, int32_t sq,
                           int32_t skv, float scale, void* stream) {
+  const CUtensorMapDataType t16 = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   if (!q || !kv) return fail("%s: null operand", what);
   if (batch <= 0 || heads <= 0 || sq <= 0 || skv <= 0) return fail("%s: bad shape", what);
   if (ldq % 8 || ldkv % 8 || ldq < heads * 64 || ldkv < 2 * heads * 64) return fail("%s: bad leading dimensions", what);
@@ -195,7 +200,7 @@ static int attention_impl(const char* what, const void* q, int32_t ldq, const vo
                               static_cast<uint64_t>(batch)};
     const uint64_t str[2] = {static_cast<uint64_t>(ldq) * 2, static_cast<uint64_t>(ldq) * 2 * sq};
     const uint32_t box[3] = {64, f3r::ATT_Q_TILE, 1};
-    if (make_tmap(&tq, q, 3, dims, str, box)) return 1;
+    if (make_tmap(&tq, q, 3, dims, str, box, t16)) return 1;
   }
   {
     // the map ends where the key range ends (the batch stride stays kv_rows_total rows): the last key block of the range
@@ -205,7 +210,7 @@ static int attention_impl(const char* what, const void* q, int32_t ldq, const vo
                               static_cast<uint64_t>(batch)};
     const uint64_t str[2] = {static_cast<uint64_t>(ldkv) * 2, static_cast<uint64_t>(ldkv) * 2 * kv_rows_total};
     const uint32_t box[3] = {64, 128, 1};
-    if (make_tmap(&tkv, kv, 3, dims, str, box)) return 1;
+    if (make_tmap(&tkv, kv, 3, dims, str, box, t16)) return 1;
   }
   f3r::AttnArgs a;
   memset(&a, 0, sizeof(a));
@@ -214,29 +219,31 @@ static int attention_impl(const char* what, const void* q, int32_t ldq, const vo
   a.scale_log2 = scale * 1.4426950408889634f;
   a.ldo = ldo; a.out = out; a.lse = lse;
   a.kv_row0 = kv_row0; a.n_split = n_split; a.part_base = part_base; a.part_o = part_o; a.part_lse = part_lse;
-  return check(f3r::launch_attention(tq, tkv, a, static_cast<cudaStream_t>(stream)), what);
+  return check(f3r::launch_attention(tq, tkv, a, f16, static_cast<cudaStream_t>(stream)), what);
 }
 
-int f3r_attention(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo, float* lse,
-                  int32_t batch, int32_t heads, int32_t sq, int32_t skv, float scale, void* stream) {
-  if (!out) return fail("f3r_attention: null operand");
-  if (ldo % 8 || ldo < heads * 64) return fail("f3r_attention: bad leading dimensions");
-  return attention_impl("f3r_attention", q, ldq, kv, ldkv, skv, 0, out, ldo, lse, nullptr, nullptr, 0, 1, batch, heads,
-                        sq, skv, scale, stream);
+static int attention_full(const char* what, int f16, const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out,
+                          int32_t ldo, float* lse, int32_t batch, int32_t heads, int32_t sq, int32_t skv, float scale,
+                          void* stream) {
+  if (!out) return fail("%s: null operand", what);
+  if (ldo % 8 || ldo < heads * 64) return fail("%s: bad leading dimensions", what);
+  return attention_impl(what, f16, q, ldq, kv, ldkv, skv, 0, out, ldo, lse, nullptr, nullptr, 0, 1, batch, heads, sq, skv,
+                        scale, stream);
 }
 
-int f3r_attention_partial(const void* q, int32_t ldq, const void* kv, int32_t ldkv, int32_t kv_rows_total,
-                          int32_t kv_row0, int32_t skv, int32_t n_split, float* part_o, float* part_lse,
-                          int32_t part_base, int32_t batch, int32_t heads, int32_t sq, float scale, void* stream) {
-  if (!part_o || !part_lse || part_base < 0) return fail("f3r_attention_partial: bad partial buffers");
-  return attention_impl("f3r_attention_partial", q, ldq, kv, ldkv, kv_rows_total, kv_row0, nullptr, 0, nullptr, part_o,
-                        part_lse, part_base, n_split, batch, heads, sq, skv, scale, stream);
+static int attention_partial(const char* what, int f16, const void* q, int32_t ldq, const void* kv, int32_t ldkv,
+                             int32_t kv_rows_total, int32_t kv_row0, int32_t skv, int32_t n_split, float* part_o,
+                             float* part_lse, int32_t part_base, int32_t batch, int32_t heads, int32_t sq, float scale,
+                             void* stream) {
+  if (!part_o || !part_lse || part_base < 0) return fail("%s: bad partial buffers", what);
+  return attention_impl(what, f16, q, ldq, kv, ldkv, kv_rows_total, kv_row0, nullptr, 0, nullptr, part_o, part_lse,
+                        part_base, n_split, batch, heads, sq, skv, scale, stream);
 }
 
-int f3r_attention_segments(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo,
-                           const int32_t* seg_off, int32_t n_seg, int32_t rows, int32_t heads, float scale,
-                           int32_t n_split, float* part_o, float* part_lse, void* stream) {
-  const char* what = "f3r_attention_segments";
+static int attention_segments(const char* what, int f16, const void* q, int32_t ldq, const void* kv, int32_t ldkv,
+                              void* out, int32_t ldo, const int32_t* seg_off, int32_t n_seg, int32_t rows, int32_t heads,
+                              float scale, int32_t n_split, float* part_o, float* part_lse, void* stream) {
+  const CUtensorMapDataType t16 = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   if (!q || !kv || !seg_off) return fail("%s: null operand", what);
   if (reinterpret_cast<uintptr_t>(seg_off) & 3) return fail("%s: seg_off not 4-byte aligned", what);
   if (n_seg <= 0 || rows <= 0 || heads <= 0) return fail("%s: bad shape", what);
@@ -257,13 +264,13 @@ int f3r_attention_segments(const void* q, int32_t ldq, const void* kv, int32_t l
     const uint64_t dims[3] = {static_cast<uint64_t>(heads) * 64, static_cast<uint64_t>(rows), 1};
     const uint64_t str[2] = {static_cast<uint64_t>(ldq) * 2, static_cast<uint64_t>(ldq) * 2 * rows};
     const uint32_t box[3] = {64, f3r::ATT_Q_TILE, 1};
-    if (make_tmap(&tq, q, 3, dims, str, box)) return 1;
+    if (make_tmap(&tq, q, 3, dims, str, box, t16)) return 1;
   }
   {
     const uint64_t dims[3] = {static_cast<uint64_t>(heads) * 128, static_cast<uint64_t>(rows), 1};
     const uint64_t str[2] = {static_cast<uint64_t>(ldkv) * 2, static_cast<uint64_t>(ldkv) * 2 * rows};
     const uint32_t box[3] = {64, 128, 1};
-    if (make_tmap(&tkv, kv, 3, dims, str, box)) return 1;
+    if (make_tmap(&tkv, kv, 3, dims, str, box, t16)) return 1;
   }
   f3r::AttnArgs a;
   memset(&a, 0, sizeof(a));
@@ -272,27 +279,80 @@ int f3r_attention_segments(const void* q, int32_t ldq, const void* kv, int32_t l
   a.ldo = ldo; a.out = out;
   a.n_split = n_split; a.part_o = part_o; a.part_lse = part_lse;
   a.seg_off = seg_off; a.n_seg = n_seg;
-  return check(f3r::launch_attention_segments(tq, tkv, a, static_cast<int>(max_tiles), static_cast<cudaStream_t>(stream)),
+  return check(f3r::launch_attention_segments(tq, tkv, a, static_cast<int>(max_tiles), f16,
+                                              static_cast<cudaStream_t>(stream)),
                what);
+}
+
+static int attention_merge(const char* what, int f16, const float* part_o, const float* part_lse, int32_t n_parts,
+                           void* out, int32_t ldo, int32_t batch, int32_t heads, int32_t sq, void* stream) {
+  if (!part_o || !part_lse || !out || n_parts < 1) return fail("%s: bad arguments", what);
+  if (ldo % 8 || ldo < heads * 64) return fail("%s: bad leading dimension", what);
+  return check(f3r::launch_attention_merge(part_o, part_lse, n_parts, batch, heads, sq, out, ldo, f16,
+                                           static_cast<cudaStream_t>(stream)), what);
+}
+
+int f3r_attention(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo, float* lse,
+                  int32_t batch, int32_t heads, int32_t sq, int32_t skv, float scale, void* stream) {
+  return attention_full("f3r_attention", 0, q, ldq, kv, ldkv, out, ldo, lse, batch, heads, sq, skv, scale, stream);
+}
+
+int f3r_attention_partial(const void* q, int32_t ldq, const void* kv, int32_t ldkv, int32_t kv_rows_total,
+                          int32_t kv_row0, int32_t skv, int32_t n_split, float* part_o, float* part_lse,
+                          int32_t part_base, int32_t batch, int32_t heads, int32_t sq, float scale, void* stream) {
+  return attention_partial("f3r_attention_partial", 0, q, ldq, kv, ldkv, kv_rows_total, kv_row0, skv, n_split, part_o,
+                           part_lse, part_base, batch, heads, sq, scale, stream);
+}
+
+int f3r_attention_segments(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo,
+                           const int32_t* seg_off, int32_t n_seg, int32_t rows, int32_t heads, float scale,
+                           int32_t n_split, float* part_o, float* part_lse, void* stream) {
+  return attention_segments("f3r_attention_segments", 0, q, ldq, kv, ldkv, out, ldo, seg_off, n_seg, rows, heads, scale,
+                            n_split, part_o, part_lse, stream);
 }
 
 int f3r_attention_merge(const float* part_o, const float* part_lse, int32_t n_parts, void* out, int32_t ldo,
                         int32_t batch, int32_t heads, int32_t sq, void* stream) {
-  if (!part_o || !part_lse || !out || n_parts < 1) return fail("f3r_attention_merge: bad arguments");
-  if (ldo % 8 || ldo < heads * 64) return fail("f3r_attention_merge: bad leading dimension");
-  return check(f3r::launch_attention_merge(part_o, part_lse, n_parts, batch, heads, sq, out, ldo,
-                                           static_cast<cudaStream_t>(stream)), "f3r_attention_merge");
+  return attention_merge("f3r_attention_merge", 0, part_o, part_lse, n_parts, out, ldo, batch, heads, sq, stream);
 }
+
+int f3r_attention_f16(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo, float* lse,
+                      int32_t batch, int32_t heads, int32_t sq, int32_t skv, float scale, void* stream) {
+  return attention_full("f3r_attention_f16", 1, q, ldq, kv, ldkv, out, ldo, lse, batch, heads, sq, skv, scale, stream);
+}
+
+int f3r_attention_partial_f16(const void* q, int32_t ldq, const void* kv, int32_t ldkv, int32_t kv_rows_total,
+                              int32_t kv_row0, int32_t skv, int32_t n_split, float* part_o, float* part_lse,
+                              int32_t part_base, int32_t batch, int32_t heads, int32_t sq, float scale, void* stream) {
+  return attention_partial("f3r_attention_partial_f16", 1, q, ldq, kv, ldkv, kv_rows_total, kv_row0, skv, n_split, part_o,
+                           part_lse, part_base, batch, heads, sq, scale, stream);
+}
+
+int f3r_attention_segments_f16(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo,
+                               const int32_t* seg_off, int32_t n_seg, int32_t rows, int32_t heads, float scale,
+                               int32_t n_split, float* part_o, float* part_lse, void* stream) {
+  return attention_segments("f3r_attention_segments_f16", 1, q, ldq, kv, ldkv, out, ldo, seg_off, n_seg, rows, heads,
+                            scale, n_split, part_o, part_lse, stream);
+}
+
+int f3r_attention_merge_f16(const float* part_o, const float* part_lse, int32_t n_parts, void* out, int32_t ldo,
+                            int32_t batch, int32_t heads, int32_t sq, void* stream) {
+  return attention_merge("f3r_attention_merge_f16", 1, part_o, part_lse, n_parts, out, ldo, batch, heads, sq, stream);
+}
+
+static bool bad_elt(int32_t elt) { return elt != f3r::ELT_BF16 && elt != f3r::ELT_F32 && elt != f3r::ELT_F16; }
 
 int f3r_layernorm(const float* x, const float* w, const float* b, void* out, int32_t out_f32, int32_t rows,
                   int32_t dim, float eps, void* stream) {
   if (!x || !w || !b || !out) return fail("f3r_layernorm: null operand");
+  if (bad_elt(out_f32)) return fail("f3r_layernorm: out_f32=%d must be 0 (bf16), 1 (fp32) or 2 (fp16)", out_f32);
   return check(f3r::launch_layernorm(x, w, b, out, out_f32, rows, dim, eps, static_cast<cudaStream_t>(stream)),
                "f3r_layernorm (dim must be one of 128,256,384,512,768,1024)");
 }
 
 int f3r_im2col_patch(const float* img, void* out, int32_t out_f32, int32_t n, int32_t h, int32_t w, void* stream) {
   if (!img || !out) return fail("f3r_im2col_patch: null operand");
+  if (bad_elt(out_f32)) return fail("f3r_im2col_patch: out_f32=%d must be 0 (bf16), 1 (fp32) or 2 (fp16)", out_f32);
   return check(f3r::launch_im2col_patch(img, out, out_f32, n, h, w, 16, static_cast<cudaStream_t>(stream)),
                "f3r_im2col_patch");
 }
@@ -307,6 +367,7 @@ int f3r_im2col3x3s2(const void* in, void* out, int32_t n, int32_t h, int32_t w, 
 int f3r_upsample2x(const void* in, void* out, int32_t f32, int32_t n, int32_t h, int32_t w, int32_t c, int32_t ho,
                    int32_t wo, void* stream) {
   if (!in || !out) return fail("f3r_upsample2x: null operand");
+  if (bad_elt(f32)) return fail("f3r_upsample2x: f32=%d must be 0 (bf16), 1 (fp32) or 2 (fp16)", f32);
   if (ho > 2 * h || wo > 2 * w) return fail("f3r_upsample2x: window larger than the x2 output");
   return check(f3r::launch_upsample2x(in, out, f32, n, h, w, c, ho, wo, 2 * h, 2 * w,
                                       static_cast<cudaStream_t>(stream)),
@@ -546,6 +607,11 @@ int f3r_f64_count_below(const double* x, int32_t n, const double* th, uint64_t* 
 int f3r_cast_bf16(const float* in, void* out, size_t count, void* stream) {
   if (!in || !out) return fail("f3r_cast_bf16: null operand");
   return check(f3r::launch_cast_bf16(in, out, count, static_cast<cudaStream_t>(stream)), "f3r_cast_bf16");
+}
+
+int f3r_cast_f16(const float* in, void* out, size_t count, void* stream) {
+  if (!in || !out) return fail("f3r_cast_f16: null operand");
+  return check(f3r::launch_cast_f16(in, out, count, static_cast<cudaStream_t>(stream)), "f3r_cast_f16");
 }
 
 }  // extern "C"

@@ -1,5 +1,6 @@
-// HBM-bound helper kernels: LayerNorm (fp32 residual stream -> bf16 GEMM operand), patch im2col, strided
-// 3x3 im2col, bilinear x2 upsample (align_corners=True), fp32 -> bf16 cast.  All use 128-bit accesses.
+// HBM-bound helper kernels: LayerNorm (fp32 residual stream -> 16-bit GEMM operand), patch im2col, strided
+// 3x3 im2col, bilinear x2 upsample (align_corners=True), fp32 -> bf16 / fp16 cast.  All use 128-bit accesses.
+// The 16-bit type is bf16 or, for the fp16 forward, fp16 (T = __half); the fp32 outputs serve the parity path.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -20,7 +21,7 @@ std::atomic<uint64_t> g_launch_count{0};
 // ---------------------------------------------------------------- LayerNorm
 // nn.LayerNorm over the last dim, biased variance, y = (x-mu)/sqrt(var+eps)*w+b.  One warp per row.
 // eps 1e-6 for encoder blocks / enc_norm / dec_norm, 1e-5 for decoder blocks (fast3r/models/fast3r.py:509,683,700).
-template <int VEC>  // dim = VEC * 128
+template <int VEC, typename T>  // dim = VEC * 128; T: the 16-bit output type
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                         const float* __restrict__ b, void* __restrict__ out,
                                                         int out_f32, int rows, float eps) {
@@ -62,33 +63,41 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
           make_float4(y0, y1, y2, y3);
     } else {
       uint2 o;
-      o.x = pack_bf16(y0, y1);
-      o.y = pack_bf16(y2, y3);
-      reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(out) + static_cast<size_t>(row) * DIM)[i * 32 + lane] = o;
+      o.x = Half16<T>::pack(y0, y1);
+      o.y = Half16<T>::pack(y2, y3);
+      reinterpret_cast<uint2*>(static_cast<T*>(out) + static_cast<size_t>(row) * DIM)[i * 32 + lane] = o;
     }
   }
 }
 
-cudaError_t launch_layernorm(const float* x, const float* w, const float* b, void* out, int out_f32, int rows,
-                             int dim, float eps, cudaStream_t stream) {
-  if (rows <= 0) return cudaSuccess;
-  decltype(&layernorm_kernel<1>) kernel;
+template <typename T>
+static cudaError_t launch_layernorm_t(const float* x, const float* w, const float* b, void* out, int out_f32, int rows,
+                                      int dim, float eps, cudaStream_t stream) {
+  decltype(&layernorm_kernel<1, T>) kernel;
   switch (dim) {
-    case 128: kernel = layernorm_kernel<1>; break;
-    case 256: kernel = layernorm_kernel<2>; break;
-    case 384: kernel = layernorm_kernel<3>; break;
-    case 512: kernel = layernorm_kernel<4>; break;
-    case 768: kernel = layernorm_kernel<6>; break;
-    case 1024: kernel = layernorm_kernel<8>; break;
+    case 128: kernel = layernorm_kernel<1, T>; break;
+    case 256: kernel = layernorm_kernel<2, T>; break;
+    case 384: kernel = layernorm_kernel<3, T>; break;
+    case 512: kernel = layernorm_kernel<4, T>; break;
+    case 768: kernel = layernorm_kernel<6, T>; break;
+    case 1024: kernel = layernorm_kernel<8, T>; break;
     default: return cudaErrorInvalidValue;
   }
   return launch(kernel, (rows + 7) / 8, 256, 0, stream, true, x, w, b, out, out_f32, rows, eps);
 }
+cudaError_t launch_layernorm(const float* x, const float* w, const float* b, void* out, int out_type, int rows,
+                             int dim, float eps, cudaStream_t stream) {
+  if (out_type != ELT_BF16 && out_type != ELT_F32 && out_type != ELT_F16) return cudaErrorInvalidValue;
+  if (rows <= 0) return cudaSuccess;
+  if (out_type == ELT_F16) return launch_layernorm_t<__half>(x, w, b, out, 0, rows, dim, eps, stream);
+  return launch_layernorm_t<__nv_bfloat16>(x, w, b, out, out_type == ELT_F32, rows, dim, eps, stream);
+}
 
 // ---------------------------------------------------------------- patch im2col
-// img fp32 (n,3,H,W) -> bf16 [n*(H/p)*(W/p), 3*p*p], k = c*p*p + ky*p + kx (Conv2d weight flattening,
-// fast3r/croco/models/blocks.py:412-414), token order y*gw + x (patch_embed.py:30-33).  p == 16.
-template <bool kF32>
+// img fp32 (n,3,H,W) -> OutT [n*(H/p)*(W/p), 3*p*p], k = c*p*p + ky*p + kx (Conv2d weight flattening,
+// fast3r/croco/models/blocks.py:412-414), token order y*gw + x (patch_embed.py:30-33).  p == 16.  OutT: float,
+// __nv_bfloat16 or __half.
+template <typename OutT>
 __global__ void __launch_bounds__(256) im2col_patch_kernel(const float* __restrict__ img, void* __restrict__ out_,
                                                            int n, int H, int W) {
   const int gh = H / 16, gw = W / 16;
@@ -103,28 +112,33 @@ __global__ void __launch_bounds__(256) im2col_patch_kernel(const float* __restri
     const float4* src = reinterpret_cast<const float4*>(
         img + ((im * 3 + c) * H + gy * 16 + ky) * static_cast<size_t>(W) + gx * 16 + kx0);
     const float4 a = __ldg(src), b = __ldg(src + 1);
-    if constexpr (kF32) {  // parity mode: the GEMM operand is hi/lo-split later
+    if constexpr (std::is_same<OutT, float>::value) {  // parity mode: the GEMM operand is hi/lo-split later
       float4* out = static_cast<float4*>(out_);
       out[2 * idx] = a; out[2 * idx + 1] = b;
     } else {
       uint4 o;
-      o.x = pack_bf16(a.x, a.y); o.y = pack_bf16(a.z, a.w);
-      o.z = pack_bf16(b.x, b.y); o.w = pack_bf16(b.z, b.w);
+      using H = Half16<OutT>;
+      o.x = H::pack(a.x, a.y); o.y = H::pack(a.z, a.w);
+      o.z = H::pack(b.x, b.y); o.w = H::pack(b.z, b.w);
       static_cast<uint4*>(out_)[idx] = o;
     }
   }
 }
-cudaError_t launch_im2col_patch(const float* img, void* out, int out_f32, int n, int H, int W, int patch,
+cudaError_t launch_im2col_patch(const float* img, void* out, int out_type, int n, int H, int W, int patch,
                                 cudaStream_t stream) {
   if (patch != 16 || H % 16 || W % 16) return cudaErrorInvalidValue;
+  if (out_type != ELT_BF16 && out_type != ELT_F32 && out_type != ELT_F16) return cudaErrorInvalidValue;
   const size_t total = static_cast<size_t>(n) * (H / 16) * (W / 16) * 96;
   if (total == 0) return cudaSuccess;
   const int grid = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
-  return launch(out_f32 ? im2col_patch_kernel<true> : im2col_patch_kernel<false>, grid, 256, 0, stream, false, img, out, n,
-                H, W);
+  auto kernel = out_type == ELT_F32   ? im2col_patch_kernel<float>
+                : out_type == ELT_F16 ? im2col_patch_kernel<__half>
+                                      : im2col_patch_kernel<__nv_bfloat16>;
+  return launch(kernel, grid, 256, 0, stream, false, img, out, n, H, W);
 }
 
-// ---------------------------------------------------------------- 3x3 stride-2 pad-1 im2col (NHWC bf16)
+// ---------------------------------------------------------------- 3x3 stride-2 pad-1 im2col (NHWC, 16-bit)
+// (copies 16-byte groups of 8 elements without looking at them: the same kernel serves bf16 and fp16)
 // out [n*Ho*Wo, 9*C], k = tap*C + c, tap = ky*3+kx  (act_postprocess.3.1, fast3r/croco/models/dpt_block.py:471-478)
 __global__ void __launch_bounds__(256) im2col3x3s2_kernel(const uint4* __restrict__ in, uint4* __restrict__ out,
                                                           int n, int H, int W, int C8, int Ho, int Wo) {
@@ -152,11 +166,12 @@ cudaError_t launch_im2col3x3s2(const void* in, void* out, int n, int H, int W, i
                 H, W, C / 8, Ho, Wo);
 }
 
-// ---------------------------------------------------------------- bilinear x2, align_corners=True (NHWC bf16)
+// ---------------------------------------------------------------- bilinear x2, align_corners=True (NHWC, 16-bit T)
 // F.interpolate(scale_factor=2, mode="bilinear", align_corners=True) (fast3r/croco/models/dpt_block.py:234-247,
 // 374): src = dst * (in-1)/(full-1), full = 2*in; only the top-left Ho x Wo window of the full output is produced
 // (Ho < full implements the crop of refinenet4's output, fast3r/dust3r/heads/dpt_head.py:69-71).
 constexpr int UPS_ROWS = 8;
+template <typename T>
 __global__ void __launch_bounds__(256) upsample2x_kernel(const uint4* __restrict__ in, uint4* __restrict__ out,
                                                          int H, int W, int C8, int c8_shift, int Ho, int Wo, float sy,
                                                          float sx) {
@@ -189,9 +204,10 @@ __global__ void __launch_bounds__(256) upsample2x_kernel(const uint4* __restrict
   uint32_t ow[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
-    const float lo = w00 * bf16_lo(aw[i]) + w01 * bf16_lo(bw[i]) + w10 * bf16_lo(dw[i]) + w11 * bf16_lo(ew[i]);
-    const float hi = w00 * bf16_hi(aw[i]) + w01 * bf16_hi(bw[i]) + w10 * bf16_hi(dw[i]) + w11 * bf16_hi(ew[i]);
-    ow[i] = pack_bf16(lo, hi);
+    using H = Half16<T>;
+    const float lo = w00 * H::lo(aw[i]) + w01 * H::lo(bw[i]) + w10 * H::lo(dw[i]) + w11 * H::lo(ew[i]);
+    const float hi = w00 * H::hi(aw[i]) + w01 * H::hi(bw[i]) + w10 * H::hi(dw[i]) + w11 * H::hi(ew[i]);
+    ow[i] = H::pack(lo, hi);
   }
   out[((im * Ho + oy) * Wo + ox) * C8 + c] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
   }
@@ -222,10 +238,11 @@ __global__ void __launch_bounds__(256) upsample2x_f32_kernel(const float4* __res
   o.w = w00 * a.w + w01 * b.w + w10 * d.w + w11 * e.w;
   out[((im * Ho + oy) * Wo + ox) * C4 + c] = o;
 }
-cudaError_t launch_upsample2x(const void* in, void* out, int f32, int n, int H, int W, int C, int Ho, int Wo, int Hfull,
+cudaError_t launch_upsample2x(const void* in, void* out, int elt, int n, int H, int W, int C, int Ho, int Wo, int Hfull,
                               int Wfull, cudaStream_t stream) {
   if (C % 8 || Hfull < 2 || Wfull < 2) return cudaErrorInvalidValue;
-  if (f32) {
+  if (elt != ELT_BF16 && elt != ELT_F32 && elt != ELT_F16) return cudaErrorInvalidValue;
+  if (elt == ELT_F32) {
     const int C4 = C / 4;
     int shift = 0;
     while ((1 << shift) < C4) ++shift;
@@ -247,26 +264,33 @@ cudaError_t launch_upsample2x(const void* in, void* out, int f32, int n, int H, 
   const float sy = static_cast<float>(H - 1) / static_cast<float>(Hfull - 1);
   const float sx = static_cast<float>(W - 1) / static_cast<float>(Wfull - 1);
   dim3 grid((Wo * C8 + 255) / 256, (Ho + UPS_ROWS - 1) / UPS_ROWS, n);
-  return launch(upsample2x_kernel, grid, 256, 0, stream, false, static_cast<const uint4*>(in), static_cast<uint4*>(out), H,
-                W, C8, shift, Ho, Wo, sy, sx);
+  return launch(elt == ELT_F16 ? upsample2x_kernel<__half> : upsample2x_kernel<__nv_bfloat16>, grid, 256, 0, stream, false,
+                static_cast<const uint4*>(in), static_cast<uint4*>(out), H, W, C8, shift, Ho, Wo, sy, sx);
 }
 
-// ---------------------------------------------------------------- fp32 -> bf16
-__global__ void __launch_bounds__(256) cast_bf16_kernel(const float4* __restrict__ in, uint2* __restrict__ out,
-                                                        size_t n4) {
+// ---------------------------------------------------------------- fp32 -> bf16 / fp16 (T)
+template <typename T>
+__global__ void __launch_bounds__(256) cast_kernel(const float4* __restrict__ in, uint2* __restrict__ out, size_t n4) {
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n4;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const float4 v = __ldg(in + i);
-    out[i] = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+    out[i] = make_uint2(Half16<T>::pack(v.x, v.y), Half16<T>::pack(v.z, v.w));
   }
 }
-cudaError_t launch_cast_bf16(const float* in, void* out, size_t n, cudaStream_t stream) {
+template <typename T>
+static cudaError_t launch_cast(const float* in, void* out, size_t n, cudaStream_t stream) {
   if (n % 4) return cudaErrorInvalidValue;
   if (n == 0) return cudaSuccess;
   const size_t n4 = n / 4;
   const int grid = static_cast<int>(n4 / 256 + 1 < 132 * 16 ? n4 / 256 + 1 : 132 * 16);
-  return launch(cast_bf16_kernel, grid, 256, 0, stream, false, reinterpret_cast<const float4*>(in),
+  return launch(cast_kernel<T>, grid, 256, 0, stream, false, reinterpret_cast<const float4*>(in),
                 static_cast<uint2*>(out), n4);
+}
+cudaError_t launch_cast_bf16(const float* in, void* out, size_t n, cudaStream_t stream) {
+  return launch_cast<__nv_bfloat16>(in, out, n, stream);
+}
+cudaError_t launch_cast_f16(const float* in, void* out, size_t n, cudaStream_t stream) {
+  return launch_cast<__half>(in, out, n, stream);
 }
 
 }  // namespace f3r

@@ -89,7 +89,8 @@ struct GemmArgs {
   float* conf;
 };
 
-cudaError_t launch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
+// f16: A, the weights and every 16-bit output / residual are fp16 instead of bf16
+cudaError_t launch_gemm(int block_n, int f16, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
                         const CUtensorMap& to0b, const GemmArgs& a, int num_sms, cudaStream_t stream);
 
 // query rows per CTA of attention_kernel: three consumer warpgroups of 64 rows (ops.ATT_Q_TILE on the Python side)
@@ -100,7 +101,7 @@ struct AttnArgs {
   int q_tiles;                // ceil(sq / ATT_Q_TILE) (attention_x3: ceil(sq / 128))
   float scale_log2;           // softmax scale * log2(e)
   int ldo;                    // row stride of out (elements)
-  void* out;                  // bf16 [batch*sq, ldo], head h at columns h*64
+  void* out;                  // 16-bit [batch*sq, ldo] (bf16, or fp16 with f16), head h at columns h*64
   float* lse;                 // optional fp32 [batch, heads, sq] log-sum-exp (natural log)
   // key range of this launch inside the kv buffer: rows [kv_row0, kv_row0 + skv) of every batch
   int kv_row0;
@@ -115,12 +116,14 @@ struct AttnArgs {
   const int* seg_off;         // device int32 [n_seg + 1]
   int n_seg;
 };
+// f16: q, kv and out are fp16 instead of bf16
 cudaError_t launch_attention_merge(const float* part_o, const float* part_lse, int n_parts, int batch, int heads, int sq,
-                                   void* out, int ldo, cudaStream_t stream);
-cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, cudaStream_t stream);
+                                   void* out, int ldo, int f16, cudaStream_t stream);
+cudaError_t launch_attention(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, int f16,
+                             cudaStream_t stream);
 // segment mode: grid of heads * n_split * max_tiles CTAs, max_tiles >= the total query tiles of all segments
 cudaError_t launch_attention_segments(const CUtensorMap& tq, const CUtensorMap& tkv, const AttnArgs& a, int max_tiles,
-                                      cudaStream_t stream);
+                                      int f16, cudaStream_t stream);
 
 // parity mode (attention_x3.cu): hi/lo-split bf16 operands, fp32 out (AttnArgs.out is float*)
 cudaError_t launch_attention_x3(const CUtensorMap& tq3, const CUtensorMap& tk3, const CUtensorMap& tv2,
@@ -130,15 +133,18 @@ cudaError_t launch_attn_split(const float* q, int ldq, const float* kv, int ldkv
 cudaError_t launch_split3(const float* in, void* out, size_t rows, int k, int relu, cudaStream_t stream);
 cudaError_t launch_add_f32(float* dst, const float* src, size_t n, cudaStream_t stream);
 
-cudaError_t launch_layernorm(const float* x, const float* w, const float* b, void* out, int out_f32, int rows,
+// element-type codes of f3r_layernorm / f3r_im2col_patch / f3r_upsample2x
+enum { ELT_BF16 = 0, ELT_F32 = 1, ELT_F16 = 2 };
+cudaError_t launch_layernorm(const float* x, const float* w, const float* b, void* out, int out_type, int rows,
                              int dim, float eps, cudaStream_t stream);
-cudaError_t launch_im2col_patch(const float* img, void* out, int out_f32, int n, int H, int W, int patch,
+cudaError_t launch_im2col_patch(const float* img, void* out, int out_type, int n, int H, int W, int patch,
                                 cudaStream_t stream);
 cudaError_t launch_im2col3x3s2(const void* in, void* out, int n, int H, int W, int C, int Ho, int Wo,
                                cudaStream_t stream);
-cudaError_t launch_upsample2x(const void* in, void* out, int f32, int n, int H, int W, int C, int Ho, int Wo,
+cudaError_t launch_upsample2x(const void* in, void* out, int elt, int n, int H, int W, int C, int Ho, int Wo,
                               int Hfull, int Wfull, cudaStream_t stream);
 cudaError_t launch_cast_bf16(const float* in, void* out, size_t n, cudaStream_t stream);
+cudaError_t launch_cast_f16(const float* in, void* out, size_t n, cudaStream_t stream);
 
 // baseline JPEG decode (jpeg.cu); both return nullptr or the reason of the failure
 const char* jpeg_probe(const uint8_t* data, size_t size, f3r_jpeg_info* info);

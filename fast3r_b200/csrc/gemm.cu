@@ -2,8 +2,8 @@
 //
 //   out[m, n] = epilogue( sum_{tap, k} A[pixel(m) + shift(tap), k] * Wt[n, tap, k] )
 //
-// A is a channels-last bf16 activation viewed as (C, W, H, NB) and fetched by 4-D TMA boxes of
-// 128 pixels x 64 channels (out-of-bounds pixels/channels are zero-filled by TMA, which gives the
+// A is a channels-last 16-bit activation (bf16, or fp16 with T = __half) viewed as (C, W, H, NB) and fetched by 4-D
+// TMA boxes of 128 pixels x 64 channels (out-of-bounds pixels/channels are zero-filled by TMA, which gives the
 // 3x3 zero padding and the K / N tails for free).  A plain linear layer is the 1-tap case with
 // W = rows.  One producer thread issues TMA into a multi-stage smem ring; two consumer warpgroups each
 // own 64 rows of the 128-row tile and accumulate in registers with wgmma (m64 x BLOCK_N x k16).
@@ -38,8 +38,8 @@ struct GemmCfg {
 // traffic (residual reads, stores) is issued in the "transposed" mapping: lane l handles 4 consecutive columns
 // (16 B fp32 / 8 B bf16) of row 4*i + l/8, i = 0..7, so one warp instruction covers 4 full 128-byte row segments.
 struct ResChunk {
-  uint4 r0[8];  // res0 piece i: 4 fp32 (uint4) or 4 bf16 (.x,.y)
-  uint2 r1[8];  // res1 piece i: 4 bf16
+  uint4 r0[8];  // res0 piece i: 4 fp32 (uint4) or 4 16-bit values (.x,.y)
+  uint2 r1[8];  // res1 piece i: 4 16-bit values
 };
 
 __device__ __forceinline__ size_t out_offset(const GemmArgs& p, int m, int col0, int img, int py, int px) {
@@ -63,11 +63,11 @@ __device__ __forceinline__ void prefetch_res(const GemmArgs& p, ResChunk& rc, si
     if (p.res0 != nullptr) {
       if (p.res0_f32) rc.r0[i] = *reinterpret_cast<const uint4*>(static_cast<const float*>(p.res0) + off);
       else {
-        const uint2 t = *reinterpret_cast<const uint2*>(static_cast<const __nv_bfloat16*>(p.res0) + off);
+        const uint2 t = *reinterpret_cast<const uint2*>(static_cast<const uint16_t*>(p.res0) + off);
         rc.r0[i].x = t.x; rc.r0[i].y = t.y;
       }
     }
-    if (p.res1 != nullptr) rc.r1[i] = *reinterpret_cast<const uint2*>(static_cast<const __nv_bfloat16*>(p.res1) + off);
+    if (p.res1 != nullptr) rc.r1[i] = *reinterpret_cast<const uint2*>(static_cast<const uint16_t*>(p.res1) + off);
   }
 }
 
@@ -155,9 +155,12 @@ __device__ __forceinline__ bool epilogue_rows(const GemmArgs& p, float (&v)[32],
   return true;
 }
 
-// Transposed part: stage the 32x32 chunk, then residual adds / activation / stores with coalesced accesses.
+// Transposed part: stage the 32x32 chunk, then residual adds / activation / stores with coalesced accesses.  T: the
+// 16-bit element type of res0 / res1 / out0 / out1 when they are not fp32.
+template <typename T>
 __device__ __forceinline__ void epilogue_store(const GemmArgs& p, const float (&v)[32], const ResChunk& rc, uint8_t* stage,
                                                int lane, int m, int col0, size_t off_row, bool ok_row) {
+  using H = Half16<T>;
   // write own row: 16-byte chunk j of row r lives at r*128 + ((j ^ (r & 7)) << 4)
 #pragma unroll
   for (int j = 0; j < 8; ++j)
@@ -180,17 +183,17 @@ __device__ __forceinline__ void epilogue_store(const GemmArgs& p, const float (&
         x0 += __uint_as_float(rc.r0[i].x); x1 += __uint_as_float(rc.r0[i].y);
         x2 += __uint_as_float(rc.r0[i].z); x3 += __uint_as_float(rc.r0[i].w);
       } else {
-        x0 += bf16_lo(rc.r0[i].x); x1 += bf16_hi(rc.r0[i].x); x2 += bf16_lo(rc.r0[i].y); x3 += bf16_hi(rc.r0[i].y);
+        x0 += H::lo(rc.r0[i].x); x1 += H::hi(rc.r0[i].x); x2 += H::lo(rc.r0[i].y); x3 += H::hi(rc.r0[i].y);
       }
     }
     if (p.res1 != nullptr) {
-      x0 += bf16_lo(rc.r1[i].x); x1 += bf16_hi(rc.r1[i].x); x2 += bf16_lo(rc.r1[i].y); x3 += bf16_hi(rc.r1[i].y);
+      x0 += H::lo(rc.r1[i].x); x1 += H::hi(rc.r1[i].x); x2 += H::lo(rc.r1[i].y); x3 += H::hi(rc.r1[i].y);
     }
-    if (p.out1 != nullptr) {  // relu(v) in bf16: operand of the next 3x3 conv of a residual unit
+    if (p.out1 != nullptr) {  // relu(v) in 16 bits: operand of the next 3x3 conv of a residual unit
       uint2 o;
-      o.x = pack_bf16(fmaxf(x0, 0.f), fmaxf(x1, 0.f));
-      o.y = pack_bf16(fmaxf(x2, 0.f), fmaxf(x3, 0.f));
-      *reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(p.out1) + off) = o;
+      o.x = H::pack(fmaxf(x0, 0.f), fmaxf(x1, 0.f));
+      o.y = H::pack(fmaxf(x2, 0.f), fmaxf(x3, 0.f));
+      *reinterpret_cast<uint2*>(static_cast<T*>(p.out1) + off) = o;
     }
     if (p.out0 == nullptr) continue;
     if (p.act == ACT_RELU) {
@@ -208,9 +211,9 @@ __device__ __forceinline__ void epilogue_store(const GemmArgs& p, const float (&
       *reinterpret_cast<float4*>(static_cast<float*>(base) + o) = make_float4(x0, x1, x2, x3);
     } else {
       uint2 q;
-      q.x = pack_bf16(x0, x1);
-      q.y = pack_bf16(x2, x3);
-      *reinterpret_cast<uint2*>(static_cast<__nv_bfloat16*>(base) + o) = q;
+      q.x = H::pack(x0, x1);
+      q.y = H::pack(x2, x3);
+      *reinterpret_cast<uint2*>(static_cast<T*>(base) + o) = q;
     }
   }
   __syncwarp();  // staging tile is rewritten by the next chunk
@@ -221,6 +224,7 @@ __device__ __forceinline__ void epilogue_store(const GemmArgs& p, const float (&
 // 16-byte stores), then one lane hands the whole 32x32 tile to the TMA unit: a store, or for x += f(x) an fp32
 // reduce-add executed by the memory system (the residual is never read by the SM).  Out-of-range rows / columns are
 // clipped by the tensor map.
+template <typename T>
 __device__ __forceinline__ void epilogue_tma(const GemmArgs& p, float (&v)[32], uint8_t* stage, int lane,
                                              const CUtensorMap* map, bool reduce, int c_col, int c_x, int c_y, int c_img) {
   if (p.act == ACT_RELU) {
@@ -241,10 +245,10 @@ __device__ __forceinline__ void epilogue_tma(const GemmArgs& p, float (&v)[32], 
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       uint4 q;
-      q.x = pack_bf16(v[8 * j + 0], v[8 * j + 1]);
-      q.y = pack_bf16(v[8 * j + 2], v[8 * j + 3]);
-      q.z = pack_bf16(v[8 * j + 4], v[8 * j + 5]);
-      q.w = pack_bf16(v[8 * j + 6], v[8 * j + 7]);
+      q.x = Half16<T>::pack(v[8 * j + 0], v[8 * j + 1]);
+      q.y = Half16<T>::pack(v[8 * j + 2], v[8 * j + 3]);
+      q.z = Half16<T>::pack(v[8 * j + 4], v[8 * j + 5]);
+      q.w = Half16<T>::pack(v[8 * j + 6], v[8 * j + 7]);
       *reinterpret_cast<uint4*>(stage + lane * 64 + ((j ^ ((lane >> 1) & 3)) << 4)) = q;
     }
   }
@@ -257,7 +261,8 @@ __device__ __forceinline__ void epilogue_tma(const GemmArgs& p, float (&v)[32], 
   }
 }
 
-template <int BLOCK_N>
+// T: the 16-bit type of A, the weights and the 16-bit outputs / residuals (__nv_bfloat16 or __half)
+template <int BLOCK_N, typename T>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
             const __grid_constant__ CUtensorMap tmap_o0, const __grid_constant__ CUtensorMap tmap_o0b,
@@ -352,9 +357,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / 16; ++k) {
-          // advance 16 bf16 = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
-          if constexpr (BLOCK_N == 256) wgmma_ss_n256<0>(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
-          else wgmma_ss_n128<0>(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+          // advance 16 elements = 32 B along K inside the 128 B swizzle row: +2 in the (addr >> 4) field
+          if constexpr (BLOCK_N == 256) wgmma_ss_n256<0, T>(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
+          else wgmma_ss_n128<0, T>(acc, a_desc + 2 * k, b_desc + 2 * k, 1u);
         }
         wgmma_commit();
         wgmma_wait<1>();  // the MMAs of the previous stage have read their operands: release that stage
@@ -402,14 +407,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           if (p.tma_epi) {
             const bool to_b = p.split_col > 0 && col0 >= p.split_col;
             const int r0 = cg * 64 + (wg_warp & 1) * 32;  // first tile row of this warp
-            epilogue_tma(p, v, stage_buf, lane, to_b ? &tmap_o0b : &tmap_o0, p.tma_epi == 2,
+            epilogue_tma<T>(p, v, stage_buf, lane, to_b ? &tmap_o0b : &tmap_o0, p.tma_epi == 2,
                          to_b ? col0 - p.split_col : col0, tx * p.bw + (r0 & (p.bw - 1)), ty * p.bh + (r0 >> p.bw_log2),
                          mt < p.num_m_tiles ? img : p.NB);
           } else {
             const size_t off = out_offset(p, m, col0, img, py, px);
             ResChunk rc;
             prefetch_res(p, rc, off, row_ok, lane);
-            epilogue_store(p, v, rc, stage_buf, lane, m, col0, off, row_ok);
+            epilogue_store<T>(p, v, rc, stage_buf, lane, m, col0, off, row_ok);
           }
         }
       }
@@ -434,18 +439,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   }
 }
 
-template <int BLOCK_N>
+template <int BLOCK_N, typename T>
 static cudaError_t launch_gemm_t(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
                                  const CUtensorMap& to0b, const GemmArgs& a, int num_sms, cudaStream_t stream) {
   const int items = a.num_m_tiles * a.num_n_tiles * a.k_split;
-  return launch(gemm_kernel<BLOCK_N>, items < num_sms ? items : num_sms, GEMM_THREADS, GemmCfg<BLOCK_N>::kSmemBytes,
+  return launch(gemm_kernel<BLOCK_N, T>, items < num_sms ? items : num_sms, GEMM_THREADS, GemmCfg<BLOCK_N>::kSmemBytes,
                 stream, true, ta, tb, to0, to0b, a);
 }
 
-cudaError_t launch_gemm(int block_n, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
+cudaError_t launch_gemm(int block_n, int f16, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to0,
                         const CUtensorMap& to0b, const GemmArgs& a, int num_sms, cudaStream_t stream) {
-  if (block_n == 256) return launch_gemm_t<256>(ta, tb, to0, to0b, a, num_sms, stream);
-  return launch_gemm_t<128>(ta, tb, to0, to0b, a, num_sms, stream);
+  if (f16) {
+    if (block_n == 256) return launch_gemm_t<256, __half>(ta, tb, to0, to0b, a, num_sms, stream);
+    return launch_gemm_t<128, __half>(ta, tb, to0, to0b, a, num_sms, stream);
+  }
+  if (block_n == 256) return launch_gemm_t<256, __nv_bfloat16>(ta, tb, to0, to0b, a, num_sms, stream);
+  return launch_gemm_t<128, __nv_bfloat16>(ta, tb, to0, to0b, a, num_sms, stream);
 }
 
 }  // namespace f3r

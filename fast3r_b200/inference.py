@@ -8,8 +8,10 @@ dtype.  Here:
   * ``"32"`` and ``torch.float32`` -> the parity path (``precision="fp32"``: fp32 activations, hi/lo-split bf16
     tensor-core products; ~1e-5 rel-L2 of the reference's fp32 result).  ``torch.float32`` is what README/demo pass
     and clearly intend fp32, although the reference then silently runs its default autocast dtype (Q1).
-  * everything else (``torch.bfloat16``, "bf16", "16", ...) -> the fast path (``precision="bf16"``: bf16 operands,
-    fp32 accumulation / residual stream / statistics), closer to fp32 than the reference's own bf16-autocast path.
+  * everything else (``torch.bfloat16``, ``torch.float16``, "bf16", "16", ...) -> the fast path (``precision="bf16"``:
+    bf16 operands, fp32 accumulation / residual stream / statistics), closer to fp32 than the reference's own
+    bf16-autocast path.  On a model set to ``precision="fp16"`` (``model.set_precision("fp16")``) the fast path runs
+    fp16 operands instead; ``torch.float16`` does not select fp16 by itself.
 Preds always come back fp32.
 """
 from __future__ import annotations
@@ -172,13 +174,16 @@ def precision_of(dtype) -> str:
 
 
 class _precision_scope:
+    """Runs the model at the precision of ``dtype`` (precision_of) for the duration of a call.  A model set to "fp16"
+    keeps it for every dtype that selects the fast path: its fast path is fp16."""
+
     def __init__(self, model, dtype):
         self.model, self.want = model, precision_of(dtype)
 
     def __enter__(self):
         self.prev = getattr(self.model, "precision", None)
         if self.prev is not None:
-            self.model.precision = self.want
+            self.model.precision = "fp16" if (self.want == "bf16" and self.prev == "fp16") else self.want
 
     def __exit__(self, *exc):
         if self.prev is not None:

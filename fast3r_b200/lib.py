@@ -14,6 +14,8 @@ LIB_PATH = os.path.join(_HERE, "libfast3r_b200.so")
 
 EPI_STORE, EPI_ROPE, EPI_IDXEMB, EPI_CONVT, EPI_FINAL = range(5)
 ACT_NONE, ACT_RELU, ACT_GELU = range(3)
+# element-type codes of f3r_layernorm / f3r_im2col_patch / f3r_upsample2x
+ELT_BF16, ELT_F32, ELT_F16 = range(3)
 
 
 class GemmDesc(C.Structure):
@@ -28,6 +30,7 @@ class GemmDesc(C.Structure):
         ("split_col", C.c_int32), ("ldo_b", C.c_int32),
         ("tok_per_img", C.c_int32), ("grid_w", C.c_int32), ("rope_cols", C.c_int32),
         ("ct_k", C.c_int32), ("ct_cout", C.c_int32),
+        ("f16", C.c_int32),
         ("bias", C.c_void_p), ("res0", C.c_void_p), ("res1", C.c_void_p),
         ("out0", C.c_void_p), ("out0b", C.c_void_p), ("out1", C.c_void_p),
         ("rope_cos", C.c_void_p), ("rope_sin", C.c_void_p),
@@ -64,11 +67,18 @@ _API = {
                                         _F32, _P]),
     "f3r_attention_segments": (C.c_int, [_P, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _F32, _I32, _P, _P, _P]),
     "f3r_attention_merge": (C.c_int, [_P, _P, _I32, _P, _I32, _I32, _I32, _I32, _P]),
+    "f3r_attention_f16": (C.c_int, [_P, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _I32, _F32, _P]),
+    "f3r_attention_partial_f16": (C.c_int, [_P, _I32, _P, _I32, _I32, _I32, _I32, _I32, _P, _P, _I32, _I32, _I32, _I32,
+                                            _F32, _P]),
+    "f3r_attention_segments_f16": (C.c_int, [_P, _I32, _P, _I32, _P, _I32, _P, _I32, _I32, _I32, _F32, _I32, _P, _P,
+                                             _P]),
+    "f3r_attention_merge_f16": (C.c_int, [_P, _P, _I32, _P, _I32, _I32, _I32, _I32, _P]),
     "f3r_layernorm": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _F32, _P]),
     "f3r_im2col_patch": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _P]),
     "f3r_im2col3x3s2": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "f3r_upsample2x": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "f3r_cast_bf16": (C.c_int, [_P, _P, _SIZE, _P]),
+    "f3r_cast_f16": (C.c_int, [_P, _P, _SIZE, _P]),
     "f3r_resample_ksize": (C.c_int, [_I32, _I32, _I32]),
     "f3r_resample_coeffs": (C.c_int, [_I32, _I32, _I32, _P, _P]),
     "f3r_ingest_rgb8": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _P, _I32, _I32, _P, _P, _I32, _P, _I32, _I32, _I32,

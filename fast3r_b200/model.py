@@ -8,7 +8,8 @@ their ``forward`` is never called.  There is no PyTorch/CPU fallback: without th
 
 Numerics: bf16 tensor-core operands, fp32 accumulation, fp32 residual stream, fp32 LayerNorm/softmax
 statistics, fp32 outputs — closer to the reference's fp32 path than the reference's own bf16-autocast path
-(SURVEY.md Appendix B).
+(SURVEY.md Appendix B).  ``set_precision("fp16")`` runs the same kernels on fp16 operands and ``"fp32"`` the parity
+path (Fast3R docstring).
 """
 from __future__ import annotations
 
@@ -33,7 +34,7 @@ except Exception:  # pragma: no cover - huggingface_hub is optional for the kern
         def __init_subclass__(cls, **kw):
             super().__init_subclass__()
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 
 
 def _plain(cfg):
@@ -192,17 +193,18 @@ class PixelwiseTaskWithDPT(nn.Module):
 # Every GEMM weight is packed as [N_out, taps, K] with K contiguous (include/fast3r_b200.h).
 class _Packed:
     """Weights packed for one numeric path, which they carry along with the GEMM dispatch of that path.
-    ``precision`` "bf16" (fast path): bf16 weights and activations.  "fp32" (parity path): fp32 activations, which the
-    GEMM splits on the fly into bf16 [hi | lo | hi] along K, against weights packed as [Whi | Whi | Wlo] (3K wide), so
-    the same kernel accumulates hi*hi + lo*hi + hi*lo in fp32 (fp32-level products on the bf16 tensor pipe)."""
+    ``precision`` "bf16" (fast path): bf16 weights and activations.  "fp16": the same with fp16 in place of bf16.
+    "fp32" (parity path): fp32 activations, which the GEMM splits on the fly into bf16 [hi | lo | hi] along K, against
+    weights packed as [Whi | Whi | Wlo] (3K wide), so the same kernel accumulates hi*hi + lo*hi + hi*lo in fp32
+    (fp32-level products on the bf16 tensor pipe)."""
 
     def __init__(self, precision: str):
         self.x3 = precision == "fp32"
-        self.adt = F32 if self.x3 else BF16  # dtype of the activations that feed a GEMM
+        self.adt = {"bf16": BF16, "fp16": F16, "fp32": F32}[precision]  # dtype of the activations that feed a GEMM
 
     def _pk(self, w: torch.Tensor) -> torch.Tensor:
         w = w.detach().to(F32)
-        hi = w.to(BF16)
+        hi = w.to(BF16 if self.x3 else self.adt)
         if not self.x3:
             return hi.contiguous()
         lo = (w - hi.float()).to(BF16)
@@ -306,7 +308,7 @@ def _require_cuda(device) -> None:
 
 
 # --------------------------------------------------------------------------- the model
-PRECISIONS = ("bf16", "fp32")
+PRECISIONS = ("bf16", "fp32", "fp16")
 
 
 class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch/fast3r", tags=["image-to-3d"]):
@@ -318,7 +320,11 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         statistics / outputs - what the reference computes under ``torch.autocast(bfloat16)``, a little closer to fp32.
       * ``"fp32"`` (parity path): the reference's no-autocast result (``inference(..., dtype="32")``,
         fast3r/dust3r/inference_multiview.py:41-49) to ~1e-5 rel-L2: activations are stored fp32 and every tensor-core
-        product is evaluated as hi*hi + lo*hi + hi*lo on bf16 pairs (3x the MMA work)."""
+        product is evaluated as hi*hi + lo*hi + hi*lo on bf16 pairs (3x the MMA work).
+      * ``"fp16"``: the fast path with fp16 in place of every bf16 tensor (3 more mantissa bits at the same tensor-core
+        rate; fp32 stays fp32) - what the reference computes under its default ``torch.autocast("cuda")`` (fp16).  A
+        16-bit activation past 65504 becomes inf, as under that autocast.  Not available on a sequence-parallel
+        (sharded) model."""
 
     def __init__(self, encoder_args: dict, decoder_args: dict, head_args: dict, freeze="none"):
         super().__init__()
@@ -548,8 +554,8 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
                 if P_.x3:
                     hooks[i + 1] = x.clone()
                 else:
-                    t = torch.empty(M, D, dtype=BF16, device=dev)
-                    ops.cast_bf16(x, t)
+                    t = torch.empty(M, D, dtype=P_.adt, device=dev)
+                    (ops.cast_f16 if P_.adt == F16 else ops.cast_bf16)(x, t)
                     hooks[i + 1] = t
         last = torch.empty(M, D, dtype=P_.adt, device=dev)
         ops.layernorm(x, P_.dec_nw, P_.dec_nb, 1e-6, last)
@@ -559,7 +565,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
     @staticmethod
     def _rcu(hw: _DPTW, x, x_relu, w, nv, h, w_, res1=None, want_relu=False):
         """y = x + conv2(relu(conv1(relu(x)))) (+ res1); returns (y, relu(y) or None).  Fast path: relu(x) arrives as
-        the bf16 tensor x_relu and relu(y) is a second epilogue output; parity path: the ReLUs are folded into the
+        the 16-bit tensor x_relu and relu(y) is a second epilogue output; parity path: the ReLUs are folded into the
         operand split of the consuming conv (x_relu / the returned relu(y) are None)."""
         dev = x.device
         t = torch.empty(nv, h, w_, 256, dtype=hw.adt, device=dev)
@@ -570,7 +576,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
             if res1 is not None:
                 ops.add_f32(y, res1)
             return y, None
-        yr = torch.empty(nv, h, w_, 256, dtype=BF16, device=dev) if want_relu else None
+        yr = torch.empty(nv, h, w_, 256, dtype=hw.adt, device=dev) if want_relu else None
         ops.gemm(t, w[2], w=w_, h=h, nb=nv, taps=9, bias=w[3], out0=y, out1=yr, res0=x, res1=res1)
         return y, yr
 
@@ -865,6 +871,9 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         ps = self.encoder.patch_size
         groups = self._shape_groups(imgs)
         sp = self.sp_group
+        if sp is not None and self.precision == "fp16":
+            raise NotImplementedError("precision='fp16' does not run on a sequence-parallel (sharded) model: its K|V "
+                                      "exchange carries bf16; use precision='bf16' or 'fp32'")
         device = views[0]["img"].device
         if sp is not None and device.type != "cuda":
             device = next(self.parameters()).device  # sharded forward: host views are uploaded per rank below

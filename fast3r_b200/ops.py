@@ -9,7 +9,8 @@ import torch
 
 from . import lib as L
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
+HALF = (BF16, F16)  # the 16-bit types of the tensor-core operands: the bf16 and the fp16 forward
 
 # Optional per-launch CUDA-event timing of the dominant kernel (bench.py's live roofline measurement).
 # When set to a list, attention() appends (batch, heads, sq, skv, start_event, end_event), recorded on the
@@ -54,6 +55,23 @@ def _chk(t: torch.Tensor, dtype, name: str):
         raise ValueError(f"{name}: must be contiguous")
 
 
+def _half(t: torch.Tensor, name: str):
+    """dtype of a 16-bit operand (bf16 or fp16): the kernels of that type run the call."""
+    if t.dtype not in HALF:
+        raise TypeError(f"{name}: expected bfloat16 or float16, got {t.dtype}")
+    return t.dtype
+
+
+def _elt(t: torch.Tensor) -> int:
+    """Element-type code (lib.ELT_*) of a bf16 / fp32 / fp16 tensor."""
+    return {BF16: L.ELT_BF16, F32: L.ELT_F32, F16: L.ELT_F16}[t.dtype]
+
+
+def _f16(name: str, t: torch.Tensor) -> str:
+    """The fp16 twin of attention entry point `name` for fp16 operands."""
+    return name + "_f16" if t.dtype == F16 else name
+
+
 def gemm(a: torch.Tensor, wt: torch.Tensor, *, w: int, h: int = 1, nb: int = 1, taps: int = 1,
          bias: Optional[torch.Tensor] = None, out0: Optional[torch.Tensor] = None,
          out1: Optional[torch.Tensor] = None, res0: Optional[torch.Tensor] = None,
@@ -62,8 +80,10 @@ def gemm(a: torch.Tensor, wt: torch.Tensor, *, w: int, h: int = 1, nb: int = 1, 
          tok_per_img: int = 0, grid_w: int = 0, rope_cols: int = 0, rope_cos=None, rope_sin=None,
          emb_table=None, emb_ids=None, ct_k: int = 0, ct_cout: int = 0, w4=None, b4=None, pts=None, conf=None):
     """Fused GEMM / implicit conv (f3r_gemm).  a: bf16 (..., K) channels-last with nb*h*w pixels;
-    wt: bf16 (N, taps, K)."""
-    _chk(a, BF16, "a"); _chk(wt, BF16, "wt")
+    wt: bf16 (N, taps, K).  With fp16 a and wt the call runs in fp16: every 16-bit output and residual is fp16 too
+    (mixing bf16 and fp16 in one call raises)."""
+    h16 = _half(a, "a")
+    _chk(a, h16, "a"); _chk(wt, h16, "wt")
     n, k = wt.shape[0], wt.shape[-1]
     assert wt.numel() == n * taps * k
     assert a.shape[-1] == k and a.numel() == nb * h * w * k, (a.shape, nb, h, w, k)
@@ -80,22 +100,27 @@ def gemm(a: torch.Tensor, wt: torch.Tensor, *, w: int, h: int = 1, nb: int = 1, 
     if bias is not None:
         _chk(bias, F32, "bias")
     d.bias = _ptr(bias)
+    d.f16 = int(h16 == F16)
     if res0 is not None:
-        assert res0.dtype in (BF16, F32) and res0.is_contiguous()
+        if res0.dtype != F32:
+            _chk(res0, h16, "res0")
+        assert res0.is_contiguous()
         d.res0_f32 = int(res0.dtype == F32)
     d.res0 = _ptr(res0)
     if res1 is not None:
-        _chk(res1, BF16, "res1")
+        _chk(res1, h16, "res1")
     d.res1 = _ptr(res1)
     if out0 is not None:
-        assert out0.dtype in (BF16, F32) and out0.is_contiguous()
+        if out0.dtype != F32:
+            _chk(out0, h16, "out0")
+        assert out0.is_contiguous()
         d.out0_f32 = int(out0.dtype == F32)
     d.out0 = _ptr(out0)
     if out0b is not None:
         assert out0 is not None and out0b.dtype == out0.dtype
     d.out0b = _ptr(out0b)
     if out1 is not None:
-        _chk(out1, BF16, "out1")
+        _chk(out1, h16, "out1")
     d.out1 = _ptr(out1)
     d.rope_cos, d.rope_sin = _ptr(rope_cos), _ptr(rope_sin)
     d.emb_table, d.emb_ids = _ptr(emb_table), _ptr(emb_ids)
@@ -161,34 +186,38 @@ def attention_partial(q: torch.Tensor, kv: torch.Tensor, part_o: torch.Tensor, p
                       n_split: int, batch: int, heads: int, sq: int, kv_rows_total: int, kv_row0: int, skv: int,
                       scale: float):
     """Attends q to the keys [kv_row0, kv_row0 + skv) of kv (batch*kv_rows_total, ldkv), cut into n_split slices; slice s
-    fills slot part_base + s of part_o (slots, batch*sq, heads*64) fp32 / part_lse (slots, batch, heads, sq) fp32."""
-    _chk(q, BF16, "q"); _chk(kv, BF16, "kv"); _chk(part_o, F32, "part_o"); _chk(part_lse, F32, "part_lse")
+    fills slot part_base + s of part_o (slots, batch*sq, heads*64) fp32 / part_lse (slots, batch, heads, sq) fp32.
+    q and kv: both bf16 or both fp16."""
+    h16 = _half(q, "q")
+    _chk(q, h16, "q"); _chk(kv, h16, "kv"); _chk(part_o, F32, "part_o"); _chk(part_lse, F32, "part_lse")
     ldq, ldkv = q.shape[-1], kv.shape[-1]
     assert q.numel() == batch * sq * ldq and kv.numel() == batch * kv_rows_total * ldkv
     slots = part_o.shape[0]
     assert part_base + n_split <= slots and part_o.numel() == slots * batch * sq * heads * 64
     assert part_lse.numel() == slots * batch * heads * sq
-    _call("f3r_attention_partial", q, _ptr(q), ldq, _ptr(kv), ldkv, kv_rows_total, kv_row0, skv, n_split, _ptr(part_o),
+    _call(_f16("f3r_attention_partial", q), q, _ptr(q), ldq, _ptr(kv), ldkv, kv_rows_total, kv_row0, skv, n_split, _ptr(part_o),
           _ptr(part_lse), part_base, batch, heads, sq, float(scale))
 
 
 def attention_merge(part_o: torch.Tensor, part_lse: torch.Tensor, n_parts: int, out: torch.Tensor, *, batch: int,
                     heads: int, sq: int):
-    _chk(part_o, F32, "part_o"); _chk(part_lse, F32, "part_lse"); _chk(out, BF16, "out")
+    _chk(part_o, F32, "part_o"); _chk(part_lse, F32, "part_lse"); _half(out, "out"); _chk(out, out.dtype, "out")
     assert out.numel() == batch * sq * out.shape[-1] and n_parts <= part_o.shape[0]
-    _call("f3r_attention_merge", out, _ptr(part_o), _ptr(part_lse), n_parts, _ptr(out), out.shape[-1], batch, heads, sq)
+    _call(_f16("f3r_attention_merge", out), out, _ptr(part_o), _ptr(part_lse), n_parts, _ptr(out), out.shape[-1], batch, heads, sq)
 
 
 def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: int, heads: int, sq: int, skv: int,
               scale: float, lse: Optional[torch.Tensor] = None, kv_split: Optional[int] = None):
-    """q (batch*sq, ldq) bf16, kv (batch*skv, ldkv) bf16 [K | V], out (batch*sq, ldo) bf16.  When the launch would
+    """q (batch*sq, ldq) bf16, kv (batch*skv, ldkv) bf16 [K | V], out (batch*sq, ldo) bf16 (or all three fp16: the
+    fp16 kernels).  When the launch would
     leave SMs idle (few query tiles), the keys are cut into slices (more CTAs) and merged (pick_kv_split).  lse (batch,
     heads, sq) fp32 receives the log-sum-exp of the scaled scores; it is written by the one-slice kernel only, so lse with
     kv_split > 1 is refused."""
     if lse is not None and kv_split is not None and kv_split > 1:
         raise ValueError("ops.attention: lse is only written without key slices (kv_split > 1 merges partials that "
                          "carry no log-sum-exp output)")
-    _chk(q, BF16, "q"); _chk(kv, BF16, "kv"); _chk(out, BF16, "out")
+    h16 = _half(q, "q")
+    _chk(q, h16, "q"); _chk(kv, h16, "kv"); _chk(out, h16, "out")
     ldq, ldkv, ldo = q.shape[-1], kv.shape[-1], out.shape[-1]
     assert q.numel() == batch * sq * ldq and kv.numel() == batch * skv * ldkv and out.numel() == batch * sq * ldo
     timer = KERNEL_TIMER
@@ -205,7 +234,7 @@ def attention(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch: in
                           kv_rows_total=skv, kv_row0=0, skv=skv, scale=scale)
         attention_merge(part_o, part_lse, ns, out, batch=batch, heads=heads, sq=sq)
     else:
-        _call("f3r_attention", q, _ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, _ptr(lse), batch, heads, sq, skv,
+        _call(_f16("f3r_attention", q), q, _ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, _ptr(lse), batch, heads, sq, skv,
               float(scale))
     if timer is not None:
         e1.record(st)
@@ -233,11 +262,12 @@ class Segments:
 def attention_segments(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, seg_off, *, heads: int, scale: float,
                        kv_split: Optional[int] = None):
     """Block-diagonal attention in one launch (f3r_attention_segments): q (rows, ldq), kv (rows, ldkv) [K | V] and out
-    (rows, ldo), bf16; the rows [seg_off[s], seg_off[s+1]) attend to those rows only, each segment exactly as
+    (rows, ldo), all bf16 or all fp16; the rows [seg_off[s], seg_off[s+1]) attend to those rows only, each segment exactly as
     attention(batch=1) over it alone with the same key split.  seg_off: a Segments, or the offsets as a host sequence.
     kv_split: key slices per segment (a segment with fewer key blocks uses one per block); None picks it with
     pick_kv_split over all the launch's query tiles."""
-    _chk(q, BF16, "q"); _chk(kv, BF16, "kv"); _chk(out, BF16, "out")
+    h16 = _half(q, "q")
+    _chk(q, h16, "q"); _chk(kv, h16, "kv"); _chk(out, h16, "out")
     if not isinstance(seg_off, Segments):
         seg_off = Segments(seg_off, q.device)
     rows = seg_off.rows
@@ -250,14 +280,15 @@ def attention_segments(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, seg
         kv_split = pick_kv_split(units, key_blocks)
     ns = max(1, min(kv_split, key_blocks))
     n_seg, dev_off = len(lens), _ptr(seg_off.device_offsets)
+    name = _f16("f3r_attention_segments", q)
     if ns > 1:
         part_o = torch.empty(ns, rows, heads * 64, dtype=F32, device=q.device)
         part_lse = torch.empty(ns, heads, rows, dtype=F32, device=q.device)
-        _call("f3r_attention_segments", q, _ptr(q), ldq, _ptr(kv), ldkv, None, 0, dev_off, n_seg, rows, heads,
+        _call(name, q, _ptr(q), ldq, _ptr(kv), ldkv, None, 0, dev_off, n_seg, rows, heads,
               float(scale), ns, _ptr(part_o), _ptr(part_lse))
         attention_merge(part_o, part_lse, ns, out, batch=1, heads=heads, sq=rows)
     else:
-        _call("f3r_attention_segments", q, _ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, dev_off, n_seg, rows, heads,
+        _call(name, q, _ptr(q), ldq, _ptr(kv), ldkv, _ptr(out), ldo, dev_off, n_seg, rows, heads,
               float(scale), 1, None, None)
 
 
@@ -275,36 +306,43 @@ def attention_x3(q: torch.Tensor, kv: torch.Tensor, out: torch.Tensor, *, batch:
 
 def layernorm(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float, out: torch.Tensor):
     _chk(x, F32, "x"); _chk(w, F32, "w"); _chk(b, F32, "b")
-    assert out.dtype in (BF16, F32) and out.is_contiguous() and out.numel() == x.numel()
+    assert out.dtype in (BF16, F32, F16) and out.is_contiguous() and out.numel() == x.numel()
     dim = x.shape[-1]
-    _call("f3r_layernorm", x, _ptr(x), _ptr(w), _ptr(b), _ptr(out), int(out.dtype == F32), x.numel() // dim, dim,
-          float(eps))
+    _call("f3r_layernorm", x, _ptr(x), _ptr(w), _ptr(b), _ptr(out), _elt(out), x.numel() // dim, dim, float(eps))
 
 
 def im2col_patch(img: torch.Tensor, out: torch.Tensor):
     _chk(img, F32, "img")
-    assert out.dtype in (BF16, F32) and out.is_contiguous()
+    assert out.dtype in (BF16, F32, F16) and out.is_contiguous()
     n, c, h, w = img.shape
     assert c == 3 and out.numel() == n * (h // 16) * (w // 16) * 768
-    _call("f3r_im2col_patch", img, _ptr(img), _ptr(out), int(out.dtype == F32), n, h, w)
+    _call("f3r_im2col_patch", img, _ptr(img), _ptr(out), _elt(out), n, h, w)
 
 
 def im2col3x3s2(x: torch.Tensor, out: torch.Tensor, n: int, h: int, w: int, c: int, ho: int, wo: int):
-    _chk(x, BF16, "x"); _chk(out, BF16, "out")
+    """x (n, h, w, c) -> out (n*ho*wo, 9*c), both bf16 or both fp16 (the kernel copies 16-bit elements)."""
+    h16 = _half(x, "x")
+    _chk(x, h16, "x"); _chk(out, h16, "out")
     assert x.numel() == n * h * w * c and out.numel() == n * ho * wo * 9 * c
     _call("f3r_im2col3x3s2", x, _ptr(x), _ptr(out), n, h, w, c, ho, wo)
 
 
 def upsample2x(x: torch.Tensor, out: torch.Tensor, n: int, h: int, w: int, c: int, ho: int, wo: int):
-    assert x.dtype in (BF16, F32) and x.dtype == out.dtype and x.is_contiguous() and out.is_contiguous()
+    assert x.dtype in (BF16, F32, F16) and x.dtype == out.dtype and x.is_contiguous() and out.is_contiguous()
     assert x.numel() == n * h * w * c and out.numel() == n * ho * wo * c
-    _call("f3r_upsample2x", x, _ptr(x), _ptr(out), int(x.dtype == F32), n, h, w, c, ho, wo)
+    _call("f3r_upsample2x", x, _ptr(x), _ptr(out), _elt(x), n, h, w, c, ho, wo)
 
 
 def cast_bf16(x: torch.Tensor, out: torch.Tensor):
     _chk(x, F32, "x"); _chk(out, BF16, "out")
     assert x.numel() == out.numel()
     _call("f3r_cast_bf16", x, _ptr(x), _ptr(out), x.numel())
+
+
+def cast_f16(x: torch.Tensor, out: torch.Tensor):
+    _chk(x, F32, "x"); _chk(out, F16, "out")
+    assert x.numel() == out.numel()
+    _call("f3r_cast_f16", x, _ptr(x), _ptr(out), x.numel())
 
 
 # ------------------------------------------------------------------ geometry tail (csrc/geometry.cu)

@@ -10,7 +10,9 @@
  *   - enqueues on the given stream and returns 0 on success, non-zero on error (text via f3r_last_error()),
  *   - is reentrant per thread (one Python thread per GPU/process, like the reference).
  *
- * Layout conventions: activations are row-major "channels-last": a token / pixel is a row; bf16 unless noted.
+ * Layout conventions: activations are row-major "channels-last": a token / pixel is a row; bf16 unless noted.  The
+ * fp16 forward uses the same entry points with fp16 in place of every bf16 tensor (f3r_gemm_desc.f16, the element-type
+ * code 2 of f3r_layernorm / f3r_im2col_patch / f3r_upsample2x, the *_f16 attention entry points, f3r_cast_f16).
  * Weights are bf16 [N_out, taps, K_in] (K contiguous); nn.Linear.weight (out,in) is already that with taps=1;
  * nn.Conv2d.weight (out,in,kh,kw) must be permuted to (out, kh*kw, in); ConvTranspose2d (in,out,k,k) to
  * ((i*k+j)*out + o, in).
@@ -34,6 +36,8 @@ enum { F3R_ACT_NONE = 0, F3R_ACT_RELU = 1, F3R_ACT_GELU = 2 };
  *   acc[m, n] = sum_{tap, k} A[pixel(m) + shift(tap), k] * Wt[n, tap, k]          (fp32 accumulation in registers)
  *   v = acc + bias[n] (+ RoPE2D | + idx-embedding row) (+ res0[m,n]) (+ res1[m,n])
  *   out1[m,n] = bf16(relu(v))   (optional);   out0[m,n] = act(v) as bf16 or fp32 (optional)
+ * With f16 = 1 every 16-bit tensor of the call (a, wt, and res0 / res1 / out0 / out0b / out1 where not fp32) is fp16
+ * instead of bf16; the products and the epilogue are the same, in fp32. 
  * Replaces: nn.Linear qkv/proj/fc1/fc2 (fast3r/croco/models/blocks.py:94-97,125-128), decoder_embed + image-index
  * embedding add (fast3r/models/fast3r.py:782-799), RoPE2D on q,k (fast3r/croco/models/pos_embed.py:162-183),
  * patch-embed conv (blocks.py:412-414), every Conv2d/ConvTranspose2d of the DPT head
@@ -53,6 +57,7 @@ typedef struct f3r_gemm_desc {
                                              IDXEMB: tok_per_img tokens share emb_ids[m / tok_per_img];
                                              tok_per_img == 0: one id per row, emb_ids[m]                     */
   int32_t ct_k, ct_cout;                  /* CONVT: kernel==stride k, out channels; n == k*k*ct_cout           */
+  int32_t f16;                            /* 0: the 16-bit tensors are bf16; 1: they are fp16                  */
   const float* bias;   /* [n] (CONVT: [ct_cout]) or NULL                                                       */
   const void* res0;    /* fp32 or bf16 [M, ldo] or NULL (may alias out0: in-place residual stream update)      */
   const void* res1;    /* bf16 [M, ldo] or NULL                                                                */
@@ -114,22 +119,38 @@ int f3r_attention_segments(const void* q, int32_t ldq, const void* kv, int32_t l
                            int32_t n_split, float* part_o, float* part_lse, void* stream);
 int f3r_attention_merge(const float* part_o, const float* part_lse, int32_t n_parts, void* out, int32_t ldo,
                         int32_t batch, int32_t heads, int32_t sq, void* stream);
+/* fp16 forms of the four attention entry points above: the same arguments and contracts, with fp16 q / kv / out in place
+ * of bf16 (P is rounded to fp16 for the PV product; statistics, partials and LSE stay fp32). */
+int f3r_attention_f16(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo, float* lse,
+                      int32_t batch, int32_t heads, int32_t sq, int32_t skv, float scale, void* stream);
+int f3r_attention_partial_f16(const void* q, int32_t ldq, const void* kv, int32_t ldkv, int32_t kv_rows_total,
+                              int32_t kv_row0, int32_t skv, int32_t n_split, float* part_o, float* part_lse,
+                              int32_t part_base, int32_t batch, int32_t heads, int32_t sq, float scale, void* stream);
+int f3r_attention_segments_f16(const void* q, int32_t ldq, const void* kv, int32_t ldkv, void* out, int32_t ldo,
+                               const int32_t* seg_off, int32_t n_seg, int32_t rows, int32_t heads, float scale,
+                               int32_t n_split, float* part_o, float* part_lse, void* stream);
+int f3r_attention_merge_f16(const float* part_o, const float* part_lse, int32_t n_parts, void* out, int32_t ldo,
+                            int32_t batch, int32_t heads, int32_t sq, void* stream);
 
-/* nn.LayerNorm over the last dim of fp32 x [rows, dim] -> bf16 (or fp32) out  (blocks.py:219,228; fast3r.py:558,805) */
+/* Element-type codes of the out_f32 / f32 arguments below: 0 = bf16, 1 = fp32, 2 = fp16. */
+/* nn.LayerNorm over the last dim of fp32 x [rows, dim] -> bf16 (or fp32 / fp16) out  (blocks.py:219,228; fast3r.py:558,805) */
 int f3r_layernorm(const float* x, const float* w, const float* b, void* out, int32_t out_f32, int32_t rows,
                   int32_t dim, float eps, void* stream);
-/* fp32 image batch (n,3,H,W) -> bf16 (or, out_f32 != 0, fp32) [n*(H/16)*(W/16), 768] patch rows
+/* fp32 image batch (n,3,H,W) -> bf16 (or, by out_f32's code, fp32 / fp16) [n*(H/16)*(W/16), 768] patch rows
  * (im2col of blocks.py:412 Conv2d k=s=16) */
 int f3r_im2col_patch(const float* img, void* out, int32_t out_f32, int32_t n, int32_t h, int32_t w, void* stream);
-/* bf16 NHWC (n,h,w,c) -> bf16 [n*ho*wo, 9*c] for the 3x3 stride-2 pad-1 conv (dpt_block.py:471-478) */
+/* bf16 NHWC (n,h,w,c) -> bf16 [n*ho*wo, 9*c] for the 3x3 stride-2 pad-1 conv (dpt_block.py:471-478); a pure copy of
+ * 16-bit elements, so fp16 in gives fp16 out */
 int f3r_im2col3x3s2(const void* in, void* out, int32_t n, int32_t h, int32_t w, int32_t c, int32_t ho, int32_t wo,
                     void* stream);
-/* bilinear x2 align_corners=True on bf16 (f32 != 0: fp32) NHWC; writes the top-left (ho, wo) window of the (2h, 2w)
+/* bilinear x2 align_corners=True on NHWC in and out of the type coded by f32 (bf16, fp32 or fp16); writes the top-left (ho, wo) window of the (2h, 2w)
  * result (dpt_block.py:234-247,374; crop of dpt_head.py:69-71) */
 int f3r_upsample2x(const void* in, void* out, int32_t f32, int32_t n, int32_t h, int32_t w, int32_t c, int32_t ho,
                    int32_t wo, void* stream);
 /* fp32 -> bf16, count multiple of 4 */
 int f3r_cast_bf16(const float* in, void* out, size_t count, void* stream);
+/* fp32 -> fp16 (round to nearest even), count multiple of 4 */
+int f3r_cast_f16(const float* in, void* out, size_t count, void* stream);
 
 /* ---- image ingest (SURVEY §8 f3): PIL.Image.resize(LANCZOS | BICUBIC) + center crop + ToTensor + Normalize(0.5, 0.5) of
  * load_images() (fast3r/dust3r/utils/image.py:68-159) on a decoded 8-bit RGB image, bit-exact with Pillow's 8-bit

@@ -1,8 +1,8 @@
 """Precision study (CPU, test infrastructure): which rounding points of the CUDA path have to go beyond bf16 for
 the north star's 1e-3 rel-L2?  Runs the PRODUCT host code over tests/abi_emulator.py with selectable rounding:
-  gemm:  'bf16' (operands rounded to bf16) | 'x3' (a = hi+lo split, 3 products) | 'fp32'
-  attn:  'bf16' (q,k,v,p rounded)          | 'x3'                                 | 'fp32'
-and prints rel-L2 vs the reference fixture (tiny) / the fp32 oracle (ViT-L width)."""
+  gemm:  'bf16' (operands rounded to bf16) | 'fp16' (rounded to fp16) | 'x3' (a = hi+lo split, 3 products) | 'fp32'
+  attn:  'bf16' (q,k,v,p,o rounded)        | 'fp16' (rounded to fp16) | 'x3'                                 | 'fp32'
+(the 'fp16' rows are the rounding points of precision="fp16") and prints rel-L2 vs the reference fixture (tiny) / the fp32 oracle (ViT-L width)."""
 import os
 import sys
 
@@ -15,10 +15,11 @@ from tests.conftest import rel_l2  # noqa: E402
 from tests.golden.synth import synth_state_dict, synth_images  # noqa: E402
 
 BF = torch.bfloat16
+ROUND = {"bf16": BF, "fp16": torch.float16}  # the 16-bit storage type of the 'bf16' / 'fp16' modes
 
 
-def r16(t):
-    return t.to(BF).float()
+def r16(t, dt=BF):
+    return t.to(dt).float()
 
 
 def split(t):
@@ -33,8 +34,8 @@ def run(model, imgs, seed, gemm_mode, attn_mode):
     orig_gemm, orig_att = E.gemm, E.attention
 
     def gemm(a, wt, **kw):
-        if gemm_mode == "bf16":
-            return orig_gemm(r16(a), r16(wt), **kw)
+        if gemm_mode in ROUND:
+            return orig_gemm(r16(a, ROUND[gemm_mode]), r16(wt, ROUND[gemm_mode]), **kw)
         if gemm_mode == "x3":  # emulate hi/lo: a*w ~ ah*wh + al*wh + ah*wl: drop al*wl
             ah, al = split(a.float())
             wh, wl = split(wt.float())
@@ -45,6 +46,16 @@ def run(model, imgs, seed, gemm_mode, attn_mode):
 
     def attention(q, kv, out, *, batch, heads, sq, skv, scale, lse=None):
         D = heads * 64
+        if attn_mode in ROUND:  # q, k, v, P and O rounded to the 16-bit type, fp32 softmax statistics
+            dt = ROUND[attn_mode]
+            qh = r16(q.reshape(batch, sq, heads, 64).transpose(1, 2).float(), dt)
+            kh = r16(kv[:, :D].reshape(batch, skv, heads, 64).transpose(1, 2).float(), dt)
+            vh = r16(kv[:, D:].reshape(batch, skv, heads, 64).transpose(1, 2).float(), dt)
+            s = (qh @ kh.transpose(-2, -1)) * scale
+            p = torch.exp(s - s.amax(-1, keepdim=True))
+            o = (r16(p, dt) @ vh) / p.sum(-1, keepdim=True)
+            out.copy_(r16(o.transpose(1, 2).reshape(batch * sq, D), dt).to(out.dtype))
+            return
         qh = q.reshape(batch, sq, heads, 64).transpose(1, 2).float()
         kh = kv[:, :D].reshape(batch, skv, heads, 64).transpose(1, 2).float()
         vh = kv[:, D:].reshape(batch, skv, heads, 64).transpose(1, 2).float()
@@ -99,7 +110,7 @@ def main():
         imgs = synth_images(2, 1, 96, 128)
         torch.manual_seed(7)
         ref, seed = O.forward(sd, enc, dec, head, imgs), 7
-    for gm, am in (("bf16", "bf16"), ("x3", "bf16"), ("x3", "qk3"), ("x3", "pv3"), ("x3", "x3"), ("fp32", "fp32")):
+    for gm, am in (("bf16", "bf16"), ("fp16", "fp16"), ("x3", "bf16"), ("x3", "qk3"), ("x3", "pv3"), ("x3", "x3"), ("fp32", "fp32")):
         preds = run(model, imgs, seed, gm, am)
         rep = {k: rel_l2(torch.cat([p[k].flatten() for p in preds]), torch.cat([p[k].float().flatten() for p in ref]))
                for k in ref[0]}
