@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 _MOVE_KEYS = "img pts3d valid_mask camera_pose camera_intrinsics F_matrix corres".split()
-_KEEP_HOST_REFS = False  # set by inference() around its loss_of_one_batch call
+_KEEP_HOST_REFS = False  # set by _forward_to_host around the model call
 
 
 def _map_leaves(obj, leaf_fn):
@@ -95,7 +95,7 @@ def check_if_same_size(imgs):
 
 class _HostSink:
     """Receives finished chunks of the model's output buffers and copies them to page-locked host memory on a side
-    stream while the model keeps computing (used by inference(); the model calls chunk_done after each head chunk)."""
+    stream while the model keeps computing (used by _forward_to_host; the model calls chunk_done per head chunk)."""
     _streams = {}
 
     def __init__(self, device):
@@ -234,13 +234,10 @@ def loss_of_one_batch(batch, model, criterion, device, precision, symmetrize_bat
     return result[ret] if ret else result
 
 
-@torch.no_grad()
-def inference(multiple_views_in_one_sample, model, device, dtype, verbose=True, profiling=False):
-    """fast3r/dust3r/inference_multiview.py:70-99."""
-    if verbose:
-        print(f">> Inference with model on {len(multiple_views_in_one_sample)} images")
-    result = []
-    multiple_shapes = not check_if_same_size(multiple_views_in_one_sample)
+def _forward_to_host(model, device, call):
+    """Runs ``call()``, which uploads views (_upload), runs the model and returns (one preds list per sample, the rest),
+    with the uploaded views' host tensors kept for _views_to_cpu and each finished head chunk streamed to page-locked
+    host memory (_HostSink).  Returns (the preds lists on the host, the rest)."""
     global _KEEP_HOST_REFS
     _KEEP_HOST_REFS = True
     dev = torch.device(device)
@@ -248,20 +245,32 @@ def inference(multiple_views_in_one_sample, model, device, dtype, verbose=True, 
     try:
         if sink is not None:
             model._host_sink = sink
-        res = loss_of_one_batch(collate_with_cat([tuple(multiple_views_in_one_sample)]), model, None, device, dtype,
-                                profiling=profiling)
+        preds, rest = call()
     finally:
         _KEEP_HOST_REFS = False
         if sink is not None:
             model._host_sink = None
-    prefilled = sink.finish() if sink is not None else None
-    profiling_info = None
-    if profiling and "profiling_info" in res:
-        profiling_info = res.pop("profiling_info")
-    res = dict(views=_views_to_cpu(res["views"]), preds=_preds_to_cpu(res["preds"], prefilled), loss=to_cpu(res["loss"]))
-    result.append(res)
-    result = collate_with_cat(result, lists=multiple_shapes)
-    if profiling and profiling_info is not None:
+    # one D2H pass over all samples: the predictions of a shape group share their device buffers across samples
+    flat = iter(_preds_to_cpu([p for sample in preds for p in sample], sink.finish() if sink is not None else None))
+    return [[next(flat) for _ in sample] for sample in preds], rest
+
+
+@torch.no_grad()
+def inference(multiple_views_in_one_sample, model, device, dtype, verbose=True, profiling=False):
+    """fast3r/dust3r/inference_multiview.py:70-99."""
+    if verbose:
+        print(f">> Inference with model on {len(multiple_views_in_one_sample)} images")
+
+    def call():
+        res = loss_of_one_batch(collate_with_cat([tuple(multiple_views_in_one_sample)]), model, None, device, dtype,
+                                profiling=profiling)
+        return [res["preds"]], res
+
+    (preds,), res = _forward_to_host(model, device, call)
+    result = collate_with_cat([dict(views=_views_to_cpu(res["views"]), preds=preds, loss=to_cpu(res["loss"]))],
+                              lists=not check_if_same_size(multiple_views_in_one_sample))
+    profiling_info = res.get("profiling_info")
+    if profiling_info is not None:
         return result, profiling_info
     return result
 
@@ -274,31 +283,19 @@ def inference_many(samples, model, device, dtype, verbose=True, profiling=False)
     The image ids are drawn per scene in scene order, as a loop of inference() calls draws them."""
     if verbose:
         print(f">> Inference with model on {len(samples)} samples, {sum(len(s) for s in samples)} images")
-    global _KEEP_HOST_REFS
-    _KEEP_HOST_REFS = True
-    dev = torch.device(device)
-    sink = _HostSink(dev) if (dev.type == "cuda" and hasattr(model, "_host_sink")) else None
     batches = [collate_with_cat([tuple(views)]) for views in samples]
-    try:
-        if sink is not None:
-            model._host_sink = sink
+
+    def call():
         for batch in batches:
-            _upload(batch, model, dev)
+            _upload(batch, model, torch.device(device))
         with _precision_scope(model, dtype):
             out = model.forward_many(batches, profiling=profiling)
-    finally:
-        _KEEP_HOST_REFS = False
-        if sink is not None:
-            model._host_sink = None
-    preds, profiling_info = out if profiling else (out, None)
-    prefilled = sink.finish() if sink is not None else None
-    # one D2H pass over all samples: the predictions of a shape group share their device buffers across samples
-    flat = _preds_to_cpu([p for sample in preds for p in sample], prefilled)
-    result, k = [], 0
-    for views, batch, sample in zip(samples, batches, preds):
-        res = dict(views=_views_to_cpu(batch), preds=flat[k:k + len(sample)], loss=None)
-        k += len(sample)
-        result.append(collate_with_cat([res], lists=not check_if_same_size(views)))
+        return out if profiling else (out, None)
+
+    preds, profiling_info = _forward_to_host(model, device, call)
+    result = [collate_with_cat([dict(views=_views_to_cpu(batch), preds=sample, loss=None)],
+                               lists=not check_if_same_size(views))
+              for views, batch, sample in zip(samples, batches, preds)]
     if profiling:
         return result, profiling_info
     return result

@@ -648,33 +648,30 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         ops.upsample2x(t, up, nv, hh, ww, 128, H, W)
         g(up, hw.h2[0], w=W, h=H, nb=nv, taps=9, bias=hw.h2[1], epi=L.EPI_FINAL, w4=hw.w4, b4=hw.b4, pts=pts, conf=conf)
 
-    def _run_heads(self, hooked, nvt, P, gh, gw, H, W, P_: _ModelW, device):
-        """All views of one resolution through the global (and local) DPT head in chunks of
-        max_parallel_views_for_head (fast3r.py:430-444).  Returns {"pts", "conf"[, "pts_local", "conf_local"]}."""
-        heads = [("", P_.head)] + ([("_local", P_.head_local)] if P_.head_local is not None else [])
-        outs = {}
-        for suffix, _hw in heads:
-            outs["pts" + suffix] = torch.empty(nvt, H, W, 3, dtype=F32, device=device)
-            outs["conf" + suffix] = torch.empty(nvt, H, W, dtype=F32, device=device)
+    def _heads(self, enc, hooked, B, P_: _ModelW, device, results):
+        """The global (and local) DPT head of every shape group, in chunks of max_parallel_views_for_head views
+        (fast3r.py:430-444); view i's predictions go into results[i]."""
+        heads = [("pts3d_in_other_view", "conf", P_.head)]
+        if P_.head_local is not None:
+            heads.append(("pts3d_local", "conf_local", P_.head_local))
         step = max(1, int(self.max_parallel_views_for_head))
         if P_.x3:
             step = min(step, 8)  # fp32 feature maps + split scratch are ~5x the bf16 footprint
-        for s in range(0, nvt, step):
-            c = min(step, nvt - s)
-            hk = [t[s * P:(s + c) * P] for t in hooked]
-            for suffix, hw in heads:
-                self._dpt(hk, c, gh, gw, H, W, hw, outs["pts" + suffix][s:s + c], outs["conf" + suffix][s:s + c])
-            if self._host_sink is not None:  # D2H of this chunk overlaps the heads of the next one (SURVEY §8 f1)
-                self._host_sink.chunk_done(list(outs.values()), s, c)
-        return outs
-
-    @staticmethod
-    def _fill_result(r, outs, j, B):
-        r["pts3d_in_other_view"] = outs["pts"][j * B:(j + 1) * B]
-        r["conf"] = outs["conf"][j * B:(j + 1) * B]
-        if "pts_local" in outs:
-            r["pts3d_local"] = outs["pts_local"][j * B:(j + 1) * B]
-            r["conf_local"] = outs["conf_local"][j * B:(j + 1) * B]
+        for ((H, W), idxs, _, P, gh, gw), hooked_g in zip(enc, hooked):
+            nvt = len(idxs) * B
+            outs = {}
+            for pts, conf, _hw in heads:
+                outs[pts] = torch.empty(nvt, H, W, 3, dtype=F32, device=device)
+                outs[conf] = torch.empty(nvt, H, W, dtype=F32, device=device)
+            for s in range(0, nvt, step):
+                c = min(step, nvt - s)
+                hk = [t[s * P:(s + c) * P] for t in hooked_g]
+                for pts, conf, hw in heads:
+                    self._dpt(hk, c, gh, gw, H, W, hw, outs[pts][s:s + c], outs[conf][s:s + c])
+                if self._host_sink is not None:  # D2H of this chunk overlaps the heads of the next one (SURVEY §8 f1)
+                    self._host_sink.chunk_done(list(outs.values()), s, c)
+            for k, i in enumerate(idxs):
+                results[i].update({key: t[k * B:(k + 1) * B] for key, t in outs.items()})
 
     # ---- portrait views (ManyAR_PatchEmbed + landscape_only heads: fast3r/dust3r/patch_embed.py:59-105,
     #      fast3r/dust3r/utils/misc.py:74-104)
@@ -717,7 +714,8 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
     def forward(self, views, profiling=False):
         self._check_forward()
         with torch.no_grad():
-            return self._forward(views, profiling)
+            preds, profiling_info = self._forward([views], profiling)
+        return (preds[0], profiling_info) if profiling else preds[0]
 
     def _landscape(self, views):
         """(batch size, images in the geometry the model runs them in, portrait flag per view) of one sample's views.
@@ -758,13 +756,6 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
             enc.append((shape, idxs) + self._encode(x, P_))
         return enc
 
-    def _heads(self, enc, hooked, B, P_: _ModelW, device, results):
-        """The DPT heads of every shape group; view i's predictions go into results[i]."""
-        for ((H, W), idxs, _, P, gh, gw), hk in zip(enc, hooked):
-            outs = self._run_heads(hk, len(idxs) * B, P, gh, gw, H, W, P_, device)
-            for k, i in enumerate(idxs):
-                self._fill_result(results[i], outs, k, B)
-
     @staticmethod
     def _to_landscape(results, portrait):
         for r, p in zip(results, portrait):
@@ -800,86 +791,46 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         Per sample, the result equals forward(sample) up to the order of fp32 sums: GEMM plans depend on the row count,
         which packing changes.  forward_many([sample]) is bit-identical to forward(sample)."""
         self._check_forward()
-        with torch.no_grad():
-            return self._forward_many(samples, profiling)
-
-    def _forward_many(self, samples, profiling=False):
         if self.sp_group is not None:
             raise NotImplementedError("forward_many does not run on a sequence-parallel (sharded) model; call forward "
                                       "per sample")
         if len(samples) == 0:
             raise ValueError("forward_many: empty sample list")
-        profiling_info = {} if profiling else None
-        t_start = time.time()
-        flat_imgs, portraits = [], []  # all views of all samples, sample after sample
-        for s, views in enumerate(samples):
-            if len(views) == 0:
-                raise ValueError(f"forward_many: sample {s} has no views")
-            B, imgs, portrait = self._landscape(views)
-            if B != 1:
-                raise ValueError(f"forward_many packs samples of batch size 1 (sample {s} has {B}); call forward for it")
-            flat_imgs += imgs
-            portraits.append(portrait)
-        device = samples[0][0]["img"].device
-        P_ = self._pack(device)
-        ps = self.encoder.patch_size
-        enc = self._encode_groups(flat_imgs, self._shape_groups(flat_imgs), device, P_)
-        if profiling:
-            _sync(device)
-            profiling_info["encode_images_time"] = time.time() - t_start
-        t1 = time.time()
-        ids = torch.cat([self.decoder.draw_image_ids(1, len(views), rank_offset=self.image_id_rank_offset)
-                         for views in samples], dim=1)  # (1, all views)
-        if profiling:
-            profiling_info["pos_emb_time"] = time.time() - t1
-            _sync(device)
-        t2 = time.time()
-        off = list(accumulate([(im.shape[-2] // ps) * (im.shape[-1] // ps) for im in flat_imgs], initial=0))
-        first = list(accumulate([len(views) for views in samples], initial=0))  # first view of each sample
-        segments = Segments([off[i] for i in first], device)
-        feats_bnp, tok_ids, to_heads = self._pack_tokens(enc, ids, off, 0, off[-1], 1, P_, device)
-        dec_out = self._decode(feats_bnp, tok_ids, 1, off[-1], 0, P_, segments=segments)
-        if profiling:
-            _sync(device)
-            profiling_info["decoder_time"] = time.time() - t2
-        t3 = time.time()
-        hooked = [[feats] + [to_head(t) for t in dec_out] for (_, _, feats, _, _, _), to_head in zip(enc, to_heads)]
-        if profiling:
-            profiling_info["head_prepare_input_time"] = time.time() - t3
-        t4 = time.time()
-        flat_results = [{} for _ in flat_imgs]
-        self._heads(enc, hooked, 1, P_, device, flat_results)
-        results = [flat_results[a:b] for a, b in zip(first, first[1:])]
-        for r, portrait in zip(results, portraits):
-            self._to_landscape(r, portrait)
-        if profiling:
-            _sync(device)
-            t_end = time.time()
-            profiling_info["head_forward_time"] = t_end - t4
-            profiling_info["total_time"] = t_end - t_start
-            return results, profiling_info
-        return results
+        with torch.no_grad():
+            preds, profiling_info = self._forward(samples, profiling, packed=True)
+        return (preds, profiling_info) if profiling else preds
 
-    def _forward(self, views, profiling=False):
+    def _forward(self, samples, profiling=False, packed=False):
+        """The forward of ``samples``, a list of view lists: (one preds list per sample, profiling_info or None).
+        forward runs one sample, batched and, on a sequence-parallel model, sharded.  ``packed`` (forward_many) runs
+        samples of batch size 1 as one decoder sequence with one attention segment per sample."""
         # (decorated with no_grad: the CUDA path has no backward kernels yet.  Training-mode FORWARD semantics - attention
         # scale 1/8, fast3r/croco/models/blocks.py:151-154 - are honoured and tested; optimisation steps are not.)
         profiling_info = {} if profiling else None
         t_start = time.time()
-        N = len(views)
-        B, imgs, portrait = self._landscape(views)
-        H, W = views[0]["img"].shape[-2:]
+        imgs, portrait = [], []  # all views of all samples, sample after sample
+        for s, views in enumerate(samples):  # forward_many's checks of a sample come with _landscape's, in sample order
+            if packed and len(views) == 0:
+                raise ValueError(f"forward_many: sample {s} has no views")
+            B, sample_imgs, sample_portrait = self._landscape(views)
+            if packed and B != 1:
+                raise ValueError(f"forward_many packs samples of batch size 1 (sample {s} has {B}); call forward for it")
+            imgs += sample_imgs
+            portrait += sample_portrait
+        N = len(imgs)
+        first = list(accumulate([len(views) for views in samples], initial=0))  # first view of each sample
         ps = self.encoder.patch_size
         groups = self._shape_groups(imgs)
         sp = self.sp_group
         if sp is not None and self.precision == "fp16":
             raise NotImplementedError("precision='fp16' does not run on a sequence-parallel (sharded) model: its K|V "
                                       "exchange carries bf16; use precision='bf16' or 'fp32'")
-        device = views[0]["img"].device
+        device = samples[0][0]["img"].device
         if sp is not None and device.type != "cuda":
             device = next(self.parameters()).device  # sharded forward: host views are uploaded per rank below
         P_ = self._pack(device)
         tokens = [(im.shape[-2] // ps) * (im.shape[-1] // ps) for im in imgs]
-        off = list(accumulate(tokens, initial=0))  # first token of each view in a sample's sequence
+        off = list(accumulate(tokens, initial=0))  # first token of each view in the decoder sequence
         # sequence parallel: contiguous views per rank, balanced by token count (views of different resolutions)
         lo, hi = (0, N) if sp is None else sp.view_range(N, tokens)
         enc = self._encode_groups(imgs, groups, device, P_, keep=lambda i: lo <= i < hi)
@@ -887,19 +838,22 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
             _sync(device)
             profiling_info["encode_images_time"] = time.time() - t_start
         t1 = time.time()
-        # image ids: same host RNG stream as the reference.  Sequence parallel: every rank consumes its own RNG draw
-        # (same side effect as the reference) but uses the ids rank 0 drew, so the result equals the single-device
-        # forward whatever the per-rank RNG states are.
-        ids = self.decoder.draw_image_ids(B, N, rank_offset=0 if sp is not None else self.image_id_rank_offset)
+        # image ids: same host RNG stream as the reference, one draw per sample in sample order.  Sequence parallel:
+        # every rank consumes its own RNG draw (same side effect as the reference) but uses the ids rank 0 drew, so the
+        # result equals the single-device forward whatever the per-rank RNG states are.
+        rank_offset = 0 if sp is not None else self.image_id_rank_offset
+        ids = torch.cat([self.decoder.draw_image_ids(B, len(views), rank_offset=rank_offset) for views in samples],
+                        dim=1)
         if sp is not None:
             ids = sp.broadcast_ids(ids, device)
         if profiling:
             profiling_info["pos_emb_time"] = time.time() - t1
             _sync(device)
         t2 = time.time()
+        segments = Segments([off[i] for i in first], device) if packed else None
         # decoder input: the tokens of each sample in (view, patch) order; to_heads[g] takes a decoder output back to
         # group g's (view, b, patch) order, the order of the head input (fast3r.py:385-398)
-        if len(groups) == 1:  # one image id per view
+        if len(groups) == 1 and not packed:  # one image id per view
             (_, idxs, feats, P, _, _), = enc
             seq, tok_per_img, ids = len(idxs) * P, P, ids[:, lo:hi].contiguous()
             if B == 1:
@@ -916,7 +870,7 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         if sp is not None:
             kvx = sp.make_kv_exchange(B, seq, self.decoder.embed_dim, rows=[off[b] - off[a] for a, b in sp.ranges],
                                       mixed=len(groups) > 1)
-        dec_out = self._decode(feats_bnp, ids, B, seq, tok_per_img, P_, kv_exchange=kvx)
+        dec_out = self._decode(feats_bnp, ids, B, seq, tok_per_img, P_, kv_exchange=kvx, segments=segments)
         if profiling:
             _sync(device)
             profiling_info["decoder_time"] = time.time() - t2
@@ -925,16 +879,16 @@ class Fast3R(nn.Module, _HubMixin, repo_url="https://github.com/facebookresearch
         if profiling:
             profiling_info["head_prepare_input_time"] = time.time() - t3
         t4 = time.time()
-        final_results = [{} for _ in range(N)]
-        self._heads(enc, hooked, B, P_, device, final_results)
-        self._to_landscape(final_results, portrait)
+        results = [{} for _ in range(N)]
+        self._heads(enc, hooked, B, P_, device, results)
+        self._to_landscape(results, portrait)
         if sp is not None and sp.gather_preds:
-            final_results = sp.gather_results(final_results, N, B, H, W, device,
-                                              shapes=[v["img"].shape[-2:] for v in views])
+            shapes = [v["img"].shape[-2:] for views in samples for v in views]
+            results = sp.gather_results(results, N, B, *shapes[0], device, shapes=shapes)
+        results = [results[a:b] for a, b in zip(first, first[1:])]
         if profiling:
             _sync(device)
             t_end = time.time()
             profiling_info["head_forward_time"] = t_end - t4
             profiling_info["total_time"] = t_end - t_start
-            return final_results, profiling_info
-        return final_results
+        return results, profiling_info
