@@ -88,14 +88,16 @@ def plan_key(d, num_sms=H100_SMS):
 # One case per plan key of the forward (reduced to the fewest views / rows that reach the same key), then a contract
 # matrix beyond the forward.  Fields besides the descriptor: ldo / ldo_b (row strides, default n / n - split_col),
 # bias (default True), tok_per_img, grid_w, rope_cols (ROPE / IDXEMB), ct_k, ct_cout (CONVT), and "key": the plan
-# key the case must reach on an H100 SXM.
+# key the case must reach on an H100 SXM.  x3 (True: the parity forward reaches the key with K = 3 k0) makes
+# tests/test_gemm_plans_gpu.py also run the case from fp32 operands through ops.gemm_x3 (a_relu: with relu(A)).
 S, R, I, T, F = L.EPI_STORE, L.EPI_ROPE, L.EPI_IDXEMB, L.EPI_CONVT, L.EPI_FINAL
 NONE, RELU, GELU = L.ACT_NONE, L.ACT_RELU, L.ACT_GELU
 
 
 def _case(name, key, **f):
     c = dict(name=name, key=key, n=None, k=None, w=None, taps=1, h=1, nb=1, epi=S, act=NONE, out0=None, out1=False, res0=None, res1=False,
-          split_col=0, bias=True, ldo=None, ldo_b=0, tok_per_img=0, grid_w=0, rope_cols=0, ct_k=0, ct_cout=0)
+          split_col=0, bias=True, ldo=None, ldo_b=0, tok_per_img=0, grid_w=0, rope_cols=0, ct_k=0, ct_cout=0, x3=False,
+          a_relu=False)
     unknown = set(f) - set(c)
     assert not unknown, unknown
     c.update(f)
@@ -107,7 +109,7 @@ def _case(name, key, **f):
 FORWARD = [
     # forward bf16 N=32 368x512
     _case("fwd00", "bn256 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- multi",
-          n=1024, k=768, w=4352, out0="f32"),
+          n=1024, k=768, w=4352, out0="f32", x3=True),
     # forward bf16 N=32 368x512
     _case("fwd01", "bn256 taps1 tma1 ks1 sbx32 ROPE NONE out0:bf16 res0:- split multi",
           n=3072, k=1024, w=1536, epi=R, out0="bf16", split_col=1024, ldo=1024, ldo_b=2048,
@@ -226,70 +228,70 @@ FORWARD = [
     # forward fp32 N=32 368x512
     _case("fwd39", "bn256 taps1 tma1 ks1 sbx32 ROPE NONE out0:f32 res0:- split multi",
           n=3072, k=3072, w=1536, epi=R, out0="f32", split_col=1024, ldo=1024, ldo_b=2048,
-          tok_per_img=736, grid_w=32, rope_cols=2048),
+          tok_per_img=736, grid_w=32, rope_cols=2048, x3=True),
     # forward fp32 N=32 368x512
     _case("fwd40", "bn256 taps1 tma1 ks1 sbx32 STORE GELU out0:f32 res0:- multi",
-          n=4096, k=3072, w=1152, act=GELU, out0="f32"),
+          n=4096, k=3072, w=1152, act=GELU, out0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd41", "bn256 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- split multi",
-          n=3072, k=3072, w=1536, out0="f32", split_col=1024, ldo=1024, ldo_b=2048),
+          n=3072, k=3072, w=1536, out0="f32", split_col=1024, ldo=1024, ldo_b=2048, x3=True),
     # forward fp32 N=32 368x512
     _case("fwd42", "bn128 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- ntail mtail",
-          n=96, k=3072, w=32, h=23, out0="f32"),
+          n=96, k=3072, w=32, h=23, out0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd43", "bn256 taps1 tma0 ks1 sbx32 CONVT NONE out0:f32 res0:- ktail mtail multi",
-          n=1536, k=288, w=32, h=23, nb=4, epi=T, out0="f32", ct_k=4, ct_cout=96),
+          n=1536, k=288, w=32, h=23, nb=4, epi=T, out0="f32", ct_k=4, ct_cout=96, x3=True),
     # forward fp32 N=32 368x512
     _case("fwd44", "bn256 taps1 tma0 ks1 sbx32 CONVT NONE out0:f32 res0:- mtail multi",
-          n=768, k=576, w=32, h=23, nb=8, epi=T, out0="f32", ct_k=2, ct_cout=192),
+          n=768, k=576, w=32, h=23, nb=8, epi=T, out0="f32", ct_k=2, ct_cout=192, x3=True),
     # forward fp32 N=32 368x512
     _case("fwd45", "bn128 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- mtail multi",
-          n=384, k=3072, w=32, h=23, nb=8, out0="f32"),
+          n=384, k=3072, w=32, h=23, nb=8, out0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd46", "bn256 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- mtail multi",
-          n=768, k=3072, w=32, h=23, nb=8, out0="f32"),
+          n=768, k=3072, w=32, h=23, nb=8, out0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd47", "bn128 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:-",
-          n=768, k=20736, w=128, out0="f32"),
+          n=768, k=20736, w=128, out0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd48", "bn256 taps9 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- ktail multi",
-          n=256, k=288, taps=9, w=128, h=92, nb=2, out0="f32", bias=False),
+          n=256, k=288, taps=9, w=128, h=92, nb=2, out0="f32", bias=False, x3=True),
     # forward fp32 N=32 368x512
     _case("fwd49", "bn256 taps9 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- multi",
-          n=256, k=576, taps=9, w=64, h=46, nb=6, out0="f32", bias=False),
+          n=256, k=576, taps=9, w=64, h=46, nb=6, out0="f32", bias=False, x3=True),
     # forward fp32 N=32 368x512
     _case("fwd50", "bn128 taps9 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- mtail",
-          n=256, k=1152, taps=9, w=32, h=23, out0="f32", bias=False),
+          n=256, k=1152, taps=9, w=32, h=23, out0="f32", bias=False, x3=True),
     # forward fp32 N=32 368x512
     _case("fwd51", "bn128 taps9 tma1 ks1 sbx16 STORE NONE out0:f32 res0:- mtail",
-          n=256, k=2304, taps=9, w=16, h=12, out0="f32", bias=False),
+          n=256, k=2304, taps=9, w=16, h=12, out0="f32", bias=False, x3=True),
     # forward fp32 N=32 368x512
     _case("fwd52", "bn128 taps9 tma1 ks1 sbx16 STORE RELU out0:f32 res0:- mtail",
-          n=256, k=768, taps=9, w=16, h=12, act=RELU, out0="f32"),
+          n=256, k=768, taps=9, w=16, h=12, act=RELU, out0="f32", x3=True, a_relu=True),
     # forward fp32 N=32 368x512
     _case("fwd53", "bn128 taps9 tma0 ks1 sbx16 STORE NONE out0:f32 res0:f32 mtail",
-          n=256, k=768, taps=9, w=16, h=12, out0="f32", res0="f32"),
+          n=256, k=768, taps=9, w=16, h=12, out0="f32", res0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd54", "bn128 taps1 tma1 ks1 sbx16 STORE NONE out0:f32 res0:- mtail",
-          n=256, k=768, w=16, h=12, out0="f32"),
+          n=256, k=768, w=16, h=12, out0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd55", "bn128 taps9 tma1 ks1 sbx32 STORE RELU out0:f32 res0:- mtail",
-          n=256, k=768, taps=9, w=32, h=23, act=RELU, out0="f32"),
+          n=256, k=768, taps=9, w=32, h=23, act=RELU, out0="f32", x3=True, a_relu=True),
     # forward fp32 N=32 368x512
     _case("fwd56", "bn128 taps9 tma0 ks1 sbx32 STORE NONE out0:f32 res0:f32 mtail",
-          n=256, k=768, taps=9, w=32, h=23, out0="f32", res0="f32"),
+          n=256, k=768, taps=9, w=32, h=23, out0="f32", res0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd57", "bn128 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- mtail",
-          n=256, k=768, w=32, h=23, out0="f32"),
+          n=256, k=768, w=32, h=23, out0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd58", "bn256 taps9 tma1 ks1 sbx32 STORE RELU out0:f32 res0:- multi",
-          n=256, k=768, taps=9, w=64, h=46, nb=6, act=RELU, out0="f32"),
+          n=256, k=768, taps=9, w=64, h=46, nb=6, act=RELU, out0="f32", x3=True, a_relu=True),
     # forward fp32 N=32 368x512
     _case("fwd59", "bn256 taps9 tma0 ks1 sbx32 STORE NONE out0:f32 res0:f32 multi",
-          n=256, k=768, taps=9, w=64, h=46, nb=6, out0="f32", res0="f32"),
+          n=256, k=768, taps=9, w=64, h=46, nb=6, out0="f32", res0="f32", x3=True),
     # forward fp32 N=32 368x512
     _case("fwd60", "bn128 taps9 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- multi",
-          n=128, k=768, taps=9, w=256, h=184, out0="f32"),
+          n=128, k=768, taps=9, w=256, h=184, out0="f32", x3=True),
     # forward bf16 N=4 368x512
     _case("fwd61", "bn128 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- multi",
           n=1024, k=768, w=2176, out0="f32"),
@@ -389,7 +391,25 @@ FORWARD = [
           n=128, k=256, taps=9, w=184, h=256, out0="bf16"),
     # forward bf16 N=1 512x368
     _case("fwd93", "bn128 taps9 tma0 ks1 sbx16 FINAL NONE out0:- res0:- multi",
-          n=128, k=128, taps=9, w=368, h=48, epi=F),
+          n=128, k=128, taps=9, w=368, h=48, epi=F),    # forward fp32 N=32 368x512 and its decoder sharded over 4 and 8 ranks: the parity path's K = 3 k of the plans above
+    # whose bf16 cases have k not divisible by 3
+    _case("fwd94", "bn256 taps1 tma1 ks1 sbx32 IDXEMB NONE out0:f32 res0:- multi",
+          n=1024, k=3072, w=4352, epi=I, out0="f32", tok_per_img=736, x3=True),
+    _case("fwd95", "bn256 taps1 tma2 ks1 sbx32 STORE NONE out0:f32 res0:f32_inplace multi",
+          n=1024, k=3072, w=8192, out0="f32", res0="f32_inplace", x3=True),
+    _case("fwd96", "bn256 taps1 tma2 ks2 sbx32 STORE NONE out0:f32 res0:f32_inplace multi",
+          n=1024, k=3072, w=5888, out0="f32", res0="f32_inplace", x3=True),
+    _case("fwd97", "bn128 taps1 tma1 ks1 sbx32 IDXEMB NONE out0:f32 res0:- multi",
+          n=1024, k=3072, w=2176, epi=I, out0="f32", tok_per_img=736, x3=True),
+    _case("fwd98", "bn128 taps1 tma2 ks2 sbx32 STORE NONE out0:f32 res0:f32_inplace multi",
+          n=1024, k=3072, w=2944, out0="f32", res0="f32_inplace", x3=True),
+    _case("fwd99", "bn128 taps9 tma0 ks1 sbx32 FINAL NONE out0:- res0:- multi",
+          n=128, k=384, taps=9, w=512, h=34, epi=F, x3=True),
+    # act_postprocess[3]'s stride-2 conv as the parity forward runs it (x3="stride2"): split3 of the 23x32 x 768 map,
+    # im2col3x3s2 of the split operand (3 * 768 channels), then the GEMM over K = 27 * 768 against the 3x3 weight packed
+    # per tap as [Whi | Whi | Wlo]
+    _case("fwd_stride2_x3", "bn128 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:-",
+          n=768, k=27 * 768, w=2 * 12 * 16, out0="f32", x3="stride2"),
 ]
 
 # ---- the contract beyond the forward
@@ -492,7 +512,13 @@ KERNEL_CHECKS = [
     _case("convT_k2", "bn128 taps1 tma0 ks1 sbx32 CONVT NONE out0:bf16 res0:- mtail",
           n=4 * 192, k=192, w=6, h=4, nb=2, epi=T, out0="bf16", ct_k=2, ct_cout=192),
     _case("final_fused", "bn128 taps9 tma0 ks1 sbx32 FINAL NONE out0:- res0:-",
-          n=128, k=128, taps=9, w=96, h=16, nb=2, epi=F),
+          n=128, k=128, taps=9, w=96, h=16, nb=2, epi=F),    # the parity path's GEMM (fp32 operands split by ops.gemm_x3)
+    _case("x3_linear", "bn128 taps1 tma1 ks1 sbx32 STORE NONE out0:f32 res0:- mtail",
+          n=512, k=3 * 1024, w=1000, out0="f32", x3=True),
+    _case("x3_linear_gelu_tails", "bn128 taps1 tma1 ks1 sbx32 STORE GELU out0:f32 res0:- ntail mtail",
+          n=96, k=3 * 256, w=333, act=GELU, out0="f32", x3=True),
+    _case("x3_conv3x3_c96_relu_res", "bn128 taps9 tma0 ks1 sbx32 STORE NONE out0:f32 res0:f32 ktail mtail",
+          n=256, k=3 * 96, taps=9, w=24, h=9, nb=2, out0="f32", res0="f32", x3=True, a_relu=True),
 ]
 
 CASES = FORWARD + CONTRACT + KERNEL_CHECKS

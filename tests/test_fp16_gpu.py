@@ -1,6 +1,6 @@
 """precision="fp16" on the GPU: every GEMM and attention launch plan of the forward per element against float64 with fp16
-operands, the fp16 element-wise kernels against torch, the fp16 forward against the reference goldens, and its launch
-count against the bf16 forward.  Needs an H100.
+operands, the fp16 forward against the reference goldens, and its launch count against the bf16 forward.  Needs an
+H100.
 
 The per-plan checks run the bf16 checks of tests/test_gemm_plans_gpu.py and tests/test_attention_plans_gpu.py with
 fp16 in place of bf16 (their module's torch.bfloat16 reads as torch.float16; ops dispatches on the dtype).  The bounds
@@ -105,69 +105,8 @@ def test_attention_case_fp16(case, regime, fp16_checks):
     APG.run_case(case, regime, seed=6000 + 2 * AP.CASES.index(case) + (regime == "grow"))
 
 
-# ------------------------------------------------------------------ element-wise kernels against torch
-def test_layernorm_fp16():
-    from fast3r_b200 import ops
-    g = torch.Generator(device="cuda").manual_seed(1)
-    for dim in (128, 256, 384, 512, 768, 1024):
-        x = torch.randn(300, dim, generator=g, device="cuda") * 3 + 1
-        w, b = torch.randn(dim, generator=g, device="cuda"), torch.randn(dim, generator=g, device="cuda")
-        out = torch.empty(300, dim, dtype=F16, device="cuda")
-        ops.layernorm(x, w, b, 1e-6, out)
-        ref = torch.nn.functional.layer_norm(x.double(), (dim,), w.double(), b.double(), 1e-6)
-        # fp32 statistics (a few ulp of fp32), then one rounding to fp16
-        assert bool(((out.double() - ref).abs() <= U16 * ref.abs() + 1e-5 * (ref.abs() + 1)).all()), dim
-        bf = torch.empty(300, dim, dtype=torch.bfloat16, device="cuda")
-        ops.layernorm(x, w, b, 1e-6, bf)  # the bf16 output is the same fp32 value rounded to bf16
-        assert rel_l2(bf, ref) > rel_l2(out, ref)
-
-
-def test_im2col_patch_fp16():
-    from fast3r_b200 import ops
-    img = torch.randn(2, 3, 48, 64, device="cuda") * 100
-    out = torch.empty(2 * 3 * 4, 768, dtype=F16, device="cuda")
-    ops.im2col_patch(img, out)
-    ref = torch.nn.functional.unfold(img, kernel_size=16, stride=16).transpose(1, 2).reshape(-1, 768)
-    assert torch.equal(out, ref.to(F16))  # a copy rounded to nearest even, as torch's .to(float16)
-
-
-def test_im2col3x3s2_copies_fp16():
-    from fast3r_b200 import ops
-    x = (torch.randn(2, 7, 9, 16, device="cuda") * 1000).to(F16)
-    out = torch.empty(2 * 4 * 5, 9 * 16, dtype=F16, device="cuda")
-    ops.im2col3x3s2(x, out, 2, 7, 9, 16, 4, 5)
-    u = torch.nn.functional.unfold(x.float().permute(0, 3, 1, 2), kernel_size=3, stride=2, padding=1)
-    ref = u.reshape(2, 16, 9, 20).permute(0, 3, 2, 1).reshape(40, 144)
-    assert torch.equal(out, ref.to(F16))
-
-
-def test_upsample2x_fp16():
-    """The fp16 kernel is the fp32 kernel's arithmetic rounded once to fp16, and close to torch's bilinear x2."""
-    from fast3r_b200 import ops
-    g = torch.Generator(device="cuda").manual_seed(2)
-    for (h, w, c, ho, wo) in ((12, 16, 256, 24, 32), (23, 32, 128, 46, 64), (6, 8, 256, 11, 16)):
-        x = (torch.randn(3, h, w, c, generator=g, device="cuda") * 50).to(F16)
-        out = torch.empty(3, ho, wo, c, dtype=F16, device="cuda")
-        ops.upsample2x(x, out, 3, h, w, c, ho, wo)
-        ref = torch.empty(3, ho, wo, c, device="cuda")
-        ops.upsample2x(x.float(), ref, 3, h, w, c, ho, wo)
-        # one rounding to fp16, plus a few fp32 ulp of the 4-term sum where the two kernels contract differently
-        bound = U16 * ref.double().abs() + 4 * 2.0 ** -24 * x.double().abs().amax()
-        assert bool(((out.double() - ref.double()).abs() <= bound).all()), (h, w, c)
-        torch_ref = torch.nn.functional.interpolate(x.double().permute(0, 3, 1, 2), scale_factor=2, mode="bilinear",
-                                                    align_corners=True)[:, :, :ho, :wo].permute(0, 2, 3, 1)
-        assert rel_l2(out, torch_ref) < 1e-3, (h, w, c)
-
-
-def test_cast_f16():
-    from fast3r_b200 import ops
-    x = torch.randn(4096 * 3, device="cuda") * torch.logspace(-9, 4.8, 4096 * 3, device="cuda")
-    x[:4] = torch.tensor([65504.0, 65520.0, -1e6, 2.0 ** -25], device="cuda")  # max, rounds to inf, inf, tie to 0
-    out = torch.empty_like(x, dtype=F16)
-    ops.cast_f16(x, out)
-    assert torch.equal(out, x.to(F16))  # bit-exact with torch (round to nearest even, overflow to inf)
-
-
+# ------------------------------------------------------------------ the 16-bit types are not mixed
+# (the fp16 element-wise kernels are checked per element against float64 by tests/test_elementwise_plans_gpu.py)
 def test_mixed_16bit_types_refused():
     from fast3r_b200 import ops
     a = torch.zeros(128, 64, dtype=F16, device="cuda")

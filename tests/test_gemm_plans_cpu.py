@@ -37,6 +37,7 @@ class Recorder:
     def gemm_x3(self, a, wt3, *, a_relu=False, **kw):  # the K = 3k GEMM over the [hi | lo | hi] split of a
         a3 = torch.empty(a.shape[:-1] + (3 * a.shape[-1],), dtype=torch.bfloat16, device=a.device)
         self.gemm(a3, wt3, **kw)
+        self.calls[-1][0]["x3"] = True
 
     def linear(self, a, wt, bias=None, **kw):
         self.gemm(a, wt, w=a.numel() // a.shape[-1], bias=bias, **kw)
@@ -124,6 +125,23 @@ def test_every_forward_plan_has_a_gpu_case(recorded):
             missing.setdefault(key, (d, where))
     assert not missing, "plan keys of the forward without a case in tests/gemm_plans.CASES:\n" + "\n".join(
         f"  {k}\n      from {where}: {d}" for k, (d, where) in sorted(missing.items()))
+
+
+def test_every_parity_forward_plan_has_an_x3_case(recorded):
+    """Every plan key of the fp32 (parity) forward has a case that runs it as the parity path computes it: fp32
+    operands split into bf16 hi / lo parts, the weight packed [Whi | Whi | Wlo] by the model's own packing
+    (tests/test_gemm_plans_gpu.run_case with x3=True).  The one GEMM of the parity forward that is not an ops.gemm_x3
+    call, the stride-2 conv over its split3 + im2col3x3s2 columns, has the case x3="stride2"."""
+    table = {c["key"] for c in GP.CASES if c["x3"]}
+    missing = {}
+    for d, where in recorded:
+        if " fp32 " in where:
+            key = GP.plan_key(d)
+            if key not in table:
+                missing.setdefault(key, (d, where))
+    assert not missing, "plan keys of the parity forward without an x3 case in tests/gemm_plans.CASES:\n" + "\n".join(
+        f"  {k}\n      from {where}: {d}" for k, (d, where) in sorted(missing.items()))
+    assert all(c["k"] % 3 == 0 for c in GP.CASES if c["x3"])
 
 
 def test_forward_never_needs_the_reduce_add_restriction(recorded):

@@ -21,6 +21,19 @@ relu(v) + b4_i carry E_o,i = |w4_i| . E + (128 + 4) 2^-22 (|w4_i| . relu|v| + |b
 kernel's fp32 norm and exp); with d = |o_xyz| and g(d) = expm1(d) / d,
     |dpts_j| <= g E_o,j + |o_j| |g'(d)| |E_o,xyz| + 2^-20 (1 + d) |pts_j|,   |dconf| <= e^c E_o,c + 2^-20 (1 + |c|) conf.
 
+Parity composition (run_case(..., x3=True), the cases with x3 set).  A and W are fp32; W is packed by the model's own
+packing (fast3r_b200.model._Packed("fp32")._lin / _conv3 / _convt: [Whi | Whi | Wlo] along K) and A is split by
+ops.gemm_x3 (split3: [hi | lo | hi], of relu(A) with a_relu).  The reference is the float64 product of the unsplit fp32
+operands through the same epilogue reference, with S taken over the unsplit operands.  With hi = bf16(x) and lo =
+bf16(x - hi) (x - hi is exact in fp32), |x - hi| <= 2^-9 |x|, |lo| <= 2^-9 |x| (1 + 2^-8) and the residual
+|x - hi - lo| <= 2^-18 |x|; so a w - (ah wh + al wh + ah wl) = al wl + ra w + (ah + al) rw is at most
+(2^-18 (1 + 2^-8)^2 + 2^-18 + 2^-18 (1 + 2^-9)) |a| |w| < 2^-16 |a| |w| per product, and
+    |v - ref| <= E + 2^-16 S,
+E as above with K_eff = taps * 3 k0 (the accumulator sees three products per element of K).  The stride-2 case
+(x3="stride2") runs the parity forward's act_postprocess[3] conv: split3 of the map, im2col3x3s2 of the split operand
+and ops.gemm over K = 27 k0 against the weight packed per tap by _conv3, compared with F.conv2d(stride 2, padding 1)
+in float64.
+
 The relative L2 error over each output is checked as well: the per-element bound catches a wrong element or tile, the
 L2 check a systematic drift that stays inside the bound.  Every element outside the region a call may write (canaries
 before and after each output, the columns beyond n for ldo > n, the other side of a column split) must keep its value."""
@@ -31,6 +44,7 @@ import torch
 import torch.nn.functional as F
 
 from tests import gemm_plans as GP
+from fast3r_b200 import lib as L_
 from tests.canaries import buffer as _buffer, check_elements, untouched as _untouched, region as _region
 
 pytestmark = pytest.mark.gpu
@@ -61,17 +75,76 @@ def _check(name, out, ref, bound, kind):
     assert rel <= REL_L2[kind], f"{name}: relative L2 error {rel:.3g} > {REL_L2[kind]}"
 
 
-def run_case(c, seed):
-    """Runs one table case through ops.gemm and checks every output element; returns nothing (raises on failure)."""
+def _x3_weight(c, rnd):
+    """fp32 weight of an x3 case in its module layout, packed by the model's own packing, and the float64 (n, taps * k0)
+    matrix the reference multiplies (tap-major like _unfold), stated from the layer definitions."""
+    from types import SimpleNamespace
+    from fast3r_b200.model import _Packed
+    P = _Packed("fp32")
+    n, taps, k0 = c["n"], c["taps"], c["k"] // 3
+    scale = (taps * k0) ** -0.5
+    if c["epi"] == L_.EPI_CONVT:  # ConvTranspose2d (in, out, k, k): column (i*k + j)*out + o of pixel -> (i, j, o)
+        kk, co = c["ct_k"], c["ct_cout"]
+        wm = rnd(k0, co, kk, kk, scale=scale)
+        col = torch.arange(n, device="cuda")
+        return P._convt(SimpleNamespace(weight=wm)), wm.double()[:, col % co, col // (kk * co), (col // co) % kk].T
+    if taps == 9:  # Conv2d (out, in, 3, 3): tap t = ky*3 + kx
+        wm = rnd(n, k0, 3, 3, scale=scale)
+        t = torch.arange(9, device="cuda")
+        return P._conv3(SimpleNamespace(weight=wm)), wm.double()[:, :, t // 3, t % 3].transpose(1, 2).reshape(n, 9 * k0)
+    wm = rnd(n, k0, scale=scale)  # Linear (out, in)
+    return P._lin(SimpleNamespace(weight=wm)), wm.double()
+
+
+def run_stride2_x3(c, seed):
+    """The parity forward's stride-2 conv (x3="stride2"), per element against float64 (module docstring)."""
+    from types import SimpleNamespace
+    from fast3r_b200 import ops
+    from fast3r_b200.model import _Packed
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    k0, n = c["k"] // 27, c["n"]
+    nv = c["w"] // (12 * 16)
+    gh, gw, h3, w3 = 23, 32, 12, 16
+    a = torch.randn(nv, gh, gw, k0, generator=g, device="cuda")
+    wm = torch.randn(n, k0, 3, 3, generator=g, device="cuda") * (9 * k0) ** -0.5
+    bias = torch.randn(n, generator=g, device="cuda")
+    w31 = _Packed("fp32")._conv3(SimpleNamespace(weight=wm))
+    a3 = torch.empty(nv, gh, gw, 3 * k0, dtype=torch.bfloat16, device="cuda")
+    ops.split3(a, a3)
+    col = torch.empty(nv * h3 * w3, 27 * k0, dtype=torch.bfloat16, device="cuda")
+    ops.im2col3x3s2(a3, col, nv, gh, gw, 3 * k0, h3, w3)
+    buf, out = _buffer((nv * h3 * w3, n), torch.float32)
+    before = buf.clone()
+    ops.gemm(col, w31.reshape(n, 1, -1), w=nv * h3 * w3, bias=bias, out0=out)
+    torch.cuda.synchronize()
+    _untouched(f"{c['name']} out0", buf, before, _region(buf.numel(), nv * h3 * w3, n, n))
+    conv = lambda x, wt: F.conv2d(x.permute(0, 3, 1, 2), wt, stride=2, padding=1).permute(0, 2, 3, 1).reshape(-1, n)  # noqa: E731,E501
+    ref = conv(a.double(), wm.double()) + bias.double()
+    S = conv(a.double().abs(), wm.double().abs()) + bias.double().abs()
+    _check(f"{c['name']} out0", out, ref, ((c["k"] + 4) * 2.0 ** -22 + 2.0 ** -16) * S, "f32")
+
+
+def run_case(c, seed, x3=False):
+    """Runs one table case through ops.gemm (x3: from fp32 operands through ops.gemm_x3, module docstring) and checks every
+    output element; returns nothing (raises on failure)."""
     from fast3r_b200 import ops, lib as L
+    if x3 and c["x3"] == "stride2":
+        return run_stride2_x3(c, seed)
     g = torch.Generator(device="cuda").manual_seed(seed)
     bf, f32 = torch.bfloat16, torch.float32
     rnd = lambda *s, scale=1.0: torch.randn(*s, generator=g, device="cuda") * scale  # noqa: E731
     n, k, taps, w, h, nb, epi, act = (c[f] for f in ("n", "k", "taps", "w", "h", "nb", "epi", "act"))
     M, keff = nb * h * w, taps * k
     final, convt = epi == L.EPI_FINAL, epi == L.EPI_CONVT
-    a = rnd(nb, h, w, k).to(bf)
-    wt = rnd(n, taps, k, scale=keff ** -0.5).to(bf)
+    if x3:
+        assert c["x3"] and k % 3 == 0 and not c["out1"] and not c["res1"], c["name"]
+        a = rnd(nb, h, w, k // 3)
+        wt, w64 = _x3_weight(c, rnd)
+        a_ref = a.clamp_min(0) if c["a_relu"] else a
+    else:
+        a = rnd(nb, h, w, k).to(bf)
+        wt = rnd(n, taps, k, scale=keff ** -0.5).to(bf)
+        a_ref, w64 = a, wt.double().reshape(n, keff)
     nbias = c["ct_cout"] if convt else n
     bias = rnd(nbias, scale=0.5 if final else 1.0) if c["bias"] else None
     split = c["split_col"]
@@ -81,8 +154,7 @@ def run_case(c, seed):
     outs = []  # (name, flat buffer, its old contents, written mask, values to check, reference key, dtype kind)
 
     # ---- float64 reference (acc, magnitude), before the outputs are written (res0 may alias out0)
-    cols = _unfold(a.double(), taps)
-    w64 = wt.double().reshape(n, keff)
+    cols = _unfold(a_ref.double(), taps)
     acc = cols @ w64.T
     mag = cols.abs() @ w64.abs().T
     del cols
@@ -123,7 +195,7 @@ def run_case(c, seed):
         r1 = rnd(M, ldo).to(bf)
         kw["res1"] = r1
         acc, mag = acc + r1.double()[:, :n], mag + r1.double()[:, :n].abs()
-    E = (keff + 4) * 2.0 ** -22 * mag
+    E = ((keff + 4) * 2.0 ** -22 + (2.0 ** -16 if x3 else 0.0)) * mag
 
     # ---- outputs
     if final:
@@ -150,7 +222,10 @@ def run_case(c, seed):
         kw["out1"] = out1
         outs.append(("out1", buf1, buf1.clone(), _region(buf1.numel(), M, ldo, n)))
 
-    ops.gemm(a, wt, **kw)
+    if x3:
+        ops.gemm_x3(a, wt, a_relu=c["a_relu"], **kw)
+    else:
+        ops.gemm(a, wt, **kw)
     torch.cuda.synchronize()
 
     # ---- checks
@@ -214,3 +289,14 @@ def test_gemm_case(case, num_sms):
     key = GP.plan_key(case, num_sms)
     assert key == case["key"], f"{case['name']} reaches plan {key!r}, not its declared {case['key']!r}"
     run_case(case, seed=1000 + GP.CASES.index(case))
+
+
+X3_CASES = [c for c in GP.CASES if c["x3"]]
+
+
+@pytest.mark.parametrize("case", X3_CASES, ids=[c["name"] for c in X3_CASES])
+def test_gemm_case_x3(case, num_sms):
+    """The case from fp32 operands as the parity forward computes it (module docstring)."""
+    key = GP.plan_key(case, num_sms)
+    assert key == case["key"], f"{case['name']} reaches plan {key!r}, not its declared {case['key']!r}"
+    run_case(case, seed=4000 + GP.CASES.index(case), x3=True)
