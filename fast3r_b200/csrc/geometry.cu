@@ -20,7 +20,9 @@ namespace f3r {
 // integer image of the floats, one more pass for its successor, then ATen's lerp.  Each CTA histograms its eighth of the
 // view (four keys per thread and iteration so that loads overlap); the eight histograms are summed through distributed
 // shared memory and every CTA derives the same digit.  Histogram updates are warp-aggregated (confidences share their
-// exponent byte, so naive shared atomics would serialise on one bin).  No global atomics, fixed result.
+// exponent byte, so naive shared atomics would serialise on one bin).  No global atomics, fixed result.  A NaN of either
+// sign makes the view's result NaN, as in ATen (its key lies above fkey(+inf) or below fkey(-inf)): the first pass flags
+// it and ORs the flag across the cluster with the histograms.
 namespace {
 
 namespace cg = cooperative_groups;
@@ -65,7 +67,7 @@ __global__ void __launch_bounds__(QT) conf_quantile_kernel(const float* __restri
   cg::cluster_group cluster = cg::this_cluster();
   __shared__ uint32_t hist[256];
   __shared__ uint32_t total[256];
-  __shared__ uint32_t s_prefix, s_k, s_cnt_le, s_min_gt;
+  __shared__ uint32_t s_prefix, s_k, s_cnt_le, s_min_gt, s_nan, s_any_nan;
   const int view = blockIdx.x / QC;
   const unsigned crank = cluster.block_rank();
   const float* c = conf + static_cast<size_t>(view) * n;
@@ -79,23 +81,38 @@ __global__ void __launch_bounds__(QT) conf_quantile_kernel(const float* __restri
   const float w = __fsub_rn(rank, static_cast<float>(lo));
 
   uint32_t prefix = 0, mask = 0, k = static_cast<uint32_t>(lo);
+  if (tid == 0) s_nan = 0;
   for (int shift = 24; shift >= 0; shift -= 8) {
     if (tid < 256) hist[tid] = 0;
     __syncthreads();
+    bool nan = false;
     for (int base = i0; base < i1; base += QT * 4) {
       uint32_t u[4];
       bool ok[4];
       load_keys4(c, base + tid * 4, i1, vec, u, ok);
 #pragma unroll
-      for (int e = 0; e < 4; ++e) hist_add(hist, ok[e] && (u[e] & mask) == prefix, (u[e] >> shift) & 255u);
+      for (int e = 0; e < 4; ++e) {
+        hist_add(hist, ok[e] && (u[e] & mask) == prefix, (u[e] >> shift) & 255u);
+        if (shift == 24) nan |= ok[e] && (u[e] > 0xff800000u || u[e] < 0x007fffffu);  // NaN: beyond fkey(+-inf)
+      }
     }
-    cluster.sync();  // all eight histograms of this view are complete
+    if (nan) s_nan = 1;
+    cluster.sync();  // all eight histograms (and NaN flags) of this view are complete
     if (tid < 256) {
       uint32_t sum = 0;
       for (unsigned r = 0; r < QC; ++r) sum += cluster.map_shared_rank(hist, r)[tid];
       total[tid] = sum;
     }
+    if (shift == 24 && tid == 256) {
+      uint32_t any = 0;
+      for (unsigned r = 0; r < QC; ++r) any |= *cluster.map_shared_rank(&s_nan, r);
+      s_any_nan = any;
+    }
     cluster.sync();  // remote reads done before any CTA clears its histogram for the next pass
+    if (shift == 24 && s_any_nan) {  // the same in every CTA of the cluster, so all leave together
+      if (crank == 0 && tid == 0) thr[view] = __uint_as_float(0x7fc00000u);
+      return;
+    }
     if (tid == 0) {
       uint32_t cum = 0;
       int d = 0;

@@ -199,7 +199,8 @@ int f3r_jpeg_decode(const uint8_t* data, size_t size, const uint8_t* data_dev, i
  *
  * f3r_conf_quantile: thr[v] = torch.quantile(conf[v].reshape(-1), q) (linear interpolation, fp32 like ATen) - the
  *   confidence threshold of align_local_pts3d_to_global (fast3r/models/multiview_dust3r_module.py:477) and of
- *   estimate_focal (:1093).  Exact: radix select on the float bit patterns.
+ *   estimate_focal (:1093).  Exact: radix select on the float bit patterns.  A view holding a NaN (either sign) gives
+ *   NaN, as torch.quantile does, so conf >= thr then selects nothing.
  * f3r_similarity_fit: per view the least-squares similarity (R, t, s), y ~ s R x + t, over the pixels with
  *   conf >= thr & valid; fewer than 3 such pixels -> over valid only; still fewer -> identity (:480-515, where the fit is
  *   roma.rigid_points_registration(x, y, compute_scaling=True)).  conf/thr and valid may be NULL (no such mask).

@@ -33,8 +33,11 @@ import numpy as np
 
 def conf_quantile(conf: np.ndarray, q: float) -> np.float32:
     """torch.quantile(conf_flat, q) for a float32 vector (ATen quantile_impl: ranks = q*(n-1) in the input dtype,
-    below = floor, above = ceil, result = below.lerp(above, rank - below))."""
+    below = floor, above = ceil, result = below.lerp(above, rank - below)).  ATen sends both ranks to the last sorted
+    element, a NaN, when the vector holds a NaN of either sign, so the result is NaN."""
     v = np.sort(np.asarray(conf, np.float32).reshape(-1))
+    if np.isnan(v).any():
+        return np.float32(np.nan)
     n = v.size
     rank = np.float32(q) * np.float32(n - 1)
     lo = int(np.floor(rank))
