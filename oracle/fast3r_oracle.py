@@ -71,13 +71,13 @@ def gelu_erf(x: Tensor) -> Tensor:
 def rope2d(t: Tensor, pos: Tensor, base: float = 100.0) -> Tensor:
     """RoPE2D.forward, fast3r/croco/models/pos_embed.py:141-183.
     t: (B, H, S, hd); pos: (B, S, 2) int (y, x).  First hd/2 dims rotate with y, last hd/2
-    with x; inside each half pair (j, j+hd/4) with angle pos * base**(-j/(hd/4))."""
+    with x; inside each half pair (j, j+hd/4) with angle pos * base**(-j/(hd/4)).  Angles in t's dtype, on t's device."""
     hd = t.shape[-1]
     D = hd // 2
-    inv_freq = 1.0 / (base ** (torch.arange(0, D, 2).float() / D))  # (D/2,)
+    inv_freq = 1.0 / (base ** (torch.arange(0, D, 2, device=t.device).to(t.dtype) / D))  # (D/2,)
 
     def rope1d(tok, p):
-        ang = p[:, None, :, None].float() * inv_freq  # (B,1,S,D/2)
+        ang = p[:, None, :, None].to(device=t.device, dtype=t.dtype) * inv_freq  # (B,1,S,D/2)
         ang = torch.cat((ang, ang), dim=-1)
         cos, sin = ang.cos(), ang.sin()
         x1, x2 = tok[..., : D // 2], tok[..., D // 2:]
@@ -126,7 +126,7 @@ def patch_embed(img: Tensor, p: Dict[str, Tensor], patch: int = 16):
     x = F.conv2d(img, p["encoder.patch_embed.proj.weight"], p["encoder.patch_embed.proj.bias"], stride=patch)
     n, C, gh, gw = x.shape
     x = x.flatten(2).transpose(1, 2)
-    yy, xx = torch.meshgrid(torch.arange(gh), torch.arange(gw), indexing="ij")
+    yy, xx = torch.meshgrid(torch.arange(gh, device=img.device), torch.arange(gw, device=img.device), indexing="ij")
     pos = torch.stack((yy.reshape(-1), xx.reshape(-1)), dim=-1)[None].expand(n, -1, -1)
     return x, pos
 
@@ -178,28 +178,30 @@ def attn_bias_scale(hd: int) -> float:
 
 def decoder(feats: Tensor, image_ids: Tensor, p: Dict[str, Tensor], depth: int, num_heads: int,
             training: bool = False, attn_bias_for_inference_enabled: bool = True,
-            taps: Optional[dict] = None) -> List[Tensor]:
+            taps: Optional[dict] = None, keep: Optional[Sequence[int]] = None) -> List[Optional[Tensor]]:
     """Fast3RDecoder.forward, fast3r/models/fast3r.py:768-808.
     feats: (B, N, P, D) encoder outputs; image_ids: (B, N) embedding-table rows per view.
     Returns the 1+depth layer outputs (B, N*P, D); last one through dec_norm (eps 1e-6);
-    decoder blocks use LN eps 1e-5 (:683), no RoPE, eval scale 0.16019 (blocks.py:151-154)."""
+    decoder blocks use LN eps 1e-5 (:683), no RoPE, eval scale 0.16019 (blocks.py:151-154).
+    ``keep``: the layer outputs to return (the others are None, so a large forward holds only the hooked ones)."""
     if feats.dim() == 4:
         B, N, P, D = feats.shape
         x = feats.reshape(B, N * P, D)
         tok_rows = image_ids[:, :, None].expand(B, N, P).reshape(B, N * P)
     else:  # (B, S, D) with one table row per token (views of different resolutions)
         x, tok_rows = feats, image_ids
-    outs = [x]
+    kept = lambda i, t: t if keep is None or i in keep else None  # noqa: E731
+    outs = [kept(0, x)]
     x = F.linear(x, p["decoder.decoder_embed.weight"], p["decoder.decoder_embed.bias"])
-    table = image_idx_table(x.shape[-1])
-    x = x + table[tok_rows]
+    table = image_idx_table(x.shape[-1]).to(x)  # the model's fp32 buffer, in the dtype of the run
+    x = x + table[tok_rows.to(x.device)]
     if taps is not None:
         taps["dec_embed"] = x.clone()
     hd = x.shape[-1] // num_heads
     scale = attn_bias_scale(hd) if (not training and attn_bias_for_inference_enabled) else hd ** -0.5
     for i in range(depth):
         x = block(x, p, f"decoder.dec_blocks.{i}.", num_heads, 1e-5, scale, None)
-        outs.append(x)
+        outs.append(kept(i + 1, x))
         if taps is not None:
             taps[f"dec_block{i}"] = x.clone()
     outs[-1] = layer_norm(x, p["decoder.dec_norm.weight"], p["decoder.dec_norm.bias"], 1e-6)
@@ -269,18 +271,35 @@ def postprocess(out: Tensor) -> Dict[str, Tensor]:
 
 
 # ----------------------------------------------------------------------------- whole path
+def _heads_in_chunks(hooked: Sequence[Tensor], H: int, W: int, p: Dict[str, Tensor], pre: str, patch: int,
+                     head_chunk: Optional[int], taps: Optional[dict] = None) -> Dict[str, Tensor]:
+    """postprocess(dpt_head(...)) over the (views*B) images of ``hooked``, ``head_chunk`` images at a time (None: all at
+    once).  The head is per-image arithmetic, so chunking only bounds the memory of the full-resolution feature maps."""
+    n = hooked[0].shape[0]
+    step = n if head_chunk is None else max(1, int(head_chunk))
+    parts = [postprocess(dpt_head([t[s:s + step] for t in hooked], H, W, p, pre, patch, taps)) for s in range(0, n, step)]
+    return parts[0] if len(parts) == 1 else {k: torch.cat([r[k] for r in parts]) for k in parts[0]}
+
+
 def forward(state_dict: Dict[str, Tensor], enc_args: dict, dec_args: dict, head_args: dict,
             imgs: Sequence[Tensor], image_ids: Optional[Tensor] = None, training: bool = False,
-            rank: int = 0, taps: Optional[dict] = None) -> List[Dict[str, Tensor]]:
+            rank: int = 0, taps: Optional[dict] = None, *, dtype: torch.dtype = torch.float32,
+            device=None, head_chunk: Optional[int] = None) -> List[Dict[str, Tensor]]:
     """Fast3R.forward for same-size views, fast3r/models/fast3r.py:302-497.
     imgs: N tensors (B,3,H,W) fp32 in [-1,1].  If ``image_ids`` is None they are drawn from the
-    global torch RNG exactly like the reference does (seed before calling)."""
-    p = {k: v.detach().float() for k, v in state_dict.items()}
+    global torch RNG exactly like the reference does (seed before calling).
+    ``dtype`` / ``device``: the weights and inputs are cast to ``dtype`` and moved to ``device`` (None: the CPU), and
+    every op runs there (torch.float64 on a GPU gives an independent high-precision reference: torch, cuBLAS and cuDNN
+    only).  The image ids are still drawn on the CPU generator.  ``head_chunk``: images per DPT-head call (None: all).
+    Predictions come back in ``dtype`` on ``device``."""
+    device = torch.device("cpu") if device is None else torch.device(device)
+    p = {k: v.detach().to(device=device, dtype=dtype) for k, v in state_dict.items()}
     N = len(imgs)
     if any(im.shape != imgs[0].shape for im in imgs):
-        return _forward_mixed(p, enc_args, dec_args, head_args, imgs, image_ids, training, rank)
+        return _forward_mixed(p, enc_args, dec_args, head_args, imgs, image_ids, training, rank, dtype, device,
+                              head_chunk)
     B, _, H, W = imgs[0].shape
-    x = torch.cat(list(imgs), dim=0).float()  # (N*B,3,H,W), view-major (fast3r.py:258)
+    x = torch.cat(list(imgs), dim=0).to(device=device, dtype=dtype)  # (N*B,3,H,W), view-major (fast3r.py:258)
     feats, _pos = encoder(x, p, enc_args["depth"], enc_args["num_heads"], taps)
     if taps is not None:
         taps["enc_out"] = feats.clone()
@@ -291,43 +310,46 @@ def forward(state_dict: Dict[str, Tensor], enc_args: dict, dec_args: dict, head_
             image_ids = draw_image_ids(B, N, rank)
         else:
             image_ids = torch.arange(N)[None].expand(B, N)
-    outs = decoder(feats, image_ids, p, dec_args["depth"], dec_args["num_heads"], training,
-                   dec_args.get("attn_bias_for_inference_enabled", True), taps)
     d = dec_args["depth"]
     hooks = [0, d * 2 // 4, d * 3 // 4, d]
+    outs = decoder(feats, image_ids.to(device), p, dec_args["depth"], dec_args["num_heads"], training,
+                   dec_args.get("attn_bias_for_inference_enabled", True), taps, keep=hooks)
     # 'B (n p) D -> (n B) p D'  (fast3r.py:385-398)
     hooked = [outs[h].reshape(B, N, P, -1).permute(1, 0, 2, 3).reshape(N * B, P, -1) for h in hooks]
     if taps is not None:
         for i, h in enumerate(hooked):
             taps[f"hook{i}"] = h.clone()
-    res = postprocess(dpt_head(hooked, H, W, p, "downstream_head.", head_args.get("patch_size", 16), taps))
+    patch = head_args.get("patch_size", 16)
+    res = _heads_in_chunks(hooked, H, W, p, "downstream_head.", patch, head_chunk, taps)
     preds = [dict() for _ in range(N)]
     for i in range(N):
         preds[i]["pts3d_in_other_view"] = res["pts3d"][i * B:(i + 1) * B]
         preds[i]["conf"] = res["conf"][i * B:(i + 1) * B]
     if head_args.get("with_local_head", False):
-        res_l = postprocess(dpt_head(hooked, H, W, p, "downstream_head_local.", head_args.get("patch_size", 16)))
+        res_l = _heads_in_chunks(hooked, H, W, p, "downstream_head_local.", patch, head_chunk)
         for i in range(N):
             preds[i]["pts3d_local"] = res_l["pts3d"][i * B:(i + 1) * B]
             preds[i]["conf_local"] = res_l["conf"][i * B:(i + 1) * B]
     return preds
 
 
-def _forward_mixed(p, enc_args, dec_args, head_args, imgs, image_ids, training, rank):
+def _forward_mixed(p, enc_args, dec_args, head_args, imgs, image_ids, training, rank, dtype, device, head_chunk):
     """Different resolutions per view: per-view encoder and heads, one decoder pass over all tokens in view order
     (fast3r/models/fast3r.py:276-294, 339-348, 364-376, 407-428)."""
     N = len(imgs)
     B = imgs[0].shape[0]
-    feats = [encoder(im.float(), p, enc_args["depth"], enc_args["num_heads"])[0] for im in imgs]  # (B, P_i, D)
+    feats = [encoder(im.to(device=device, dtype=dtype), p, enc_args["depth"], enc_args["num_heads"])[0]
+             for im in imgs]  # (B, P_i, D)
     if image_ids is None:
         image_ids = draw_image_ids(B, N, rank) if dec_args.get("random_image_idx_embedding", True) \
             else torch.arange(N)[None].expand(B, N)
     x = torch.cat(feats, dim=1)
+    image_ids = image_ids.to(device)
     tok_rows = torch.cat([image_ids[:, i:i + 1].expand(B, f.shape[1]) for i, f in enumerate(feats)], dim=1)
-    outs = decoder(x, tok_rows, p, dec_args["depth"], dec_args["num_heads"], training,
-                   dec_args.get("attn_bias_for_inference_enabled", True))
     d = dec_args["depth"]
     hooks = [0, d * 2 // 4, d * 3 // 4, d]
+    outs = decoder(x, tok_rows, p, dec_args["depth"], dec_args["num_heads"], training,
+                   dec_args.get("attn_bias_for_inference_enabled", True), keep=hooks)
     preds = []
     off = 0
     for i, im in enumerate(imgs):
@@ -335,10 +357,10 @@ def _forward_mixed(p, enc_args, dec_args, head_args, imgs, image_ids, training, 
         hooked = [outs[h][:, off:off + P_i] for h in hooks]
         off += P_i
         H, W = im.shape[-2:]
-        r = postprocess(dpt_head(hooked, H, W, p, "downstream_head.", head_args.get("patch_size", 16)))
+        r = _heads_in_chunks(hooked, H, W, p, "downstream_head.", head_args.get("patch_size", 16), head_chunk)
         pr = dict(pts3d_in_other_view=r["pts3d"], conf=r["conf"])
         if head_args.get("with_local_head", False):
-            rl = postprocess(dpt_head(hooked, H, W, p, "downstream_head_local.", head_args.get("patch_size", 16)))
+            rl = _heads_in_chunks(hooked, H, W, p, "downstream_head_local.", head_args.get("patch_size", 16), head_chunk)
             pr.update(pts3d_local=rl["pts3d"], conf_local=rl["conf"])
         preds.append(pr)
     return preds
