@@ -583,11 +583,15 @@ __global__ void f64_mean_final_kernel(const double* __restrict__ part, int n, do
   *out = n > 0 ? t / n : NAN;
 }
 
-// exact order statistic: 8 passes of an 8-bit radix select on the order-preserving 64-bit image
+// exact order statistic: 8 passes of an 8-bit radix select on the order-preserving 64-bit image.  pc_dkey puts a NaN
+// above +inf (sign clear) or below -inf (sign set); numpy.median returns NaN if any element is NaN, so the first pass
+// flags such keys and the result is NaN.
 struct SelState {
   unsigned long long prefix, mask, min_gt;
-  unsigned int k, cnt_le;
+  unsigned int k, cnt_le, nan;
 };
+constexpr unsigned long long KEY_PINF = 0xfff0000000000000ull;  // pc_dkey(+inf)
+constexpr unsigned long long KEY_NINF = 0x000fffffffffffffull;  // pc_dkey(-inf)
 
 __global__ void sel_init_kernel(SelState* s, uint32_t* hist, int k) {
   hist[threadIdx.x] = 0;
@@ -597,10 +601,11 @@ __global__ void sel_init_kernel(SelState* s, uint32_t* hist, int k) {
     s->k = static_cast<unsigned>(k);
     s->min_gt = ~0ull;
     s->cnt_le = 0;
+    s->nan = 0;
   }
 }
 
-__global__ void __launch_bounds__(RED_T) sel_hist_kernel(const double* __restrict__ x, int n, const SelState* __restrict__ s,
+__global__ void __launch_bounds__(RED_T) sel_hist_kernel(const double* __restrict__ x, int n, SelState* __restrict__ s,
                                                          uint32_t* __restrict__ hist, int shift) {
   __shared__ uint32_t h[256];
   h[threadIdx.x] = 0;
@@ -608,12 +613,15 @@ __global__ void __launch_bounds__(RED_T) sel_hist_kernel(const double* __restric
   const unsigned long long prefix = s->prefix, mask = s->mask;
   const long long stride = static_cast<long long>(gridDim.x) * RED_T;
   const long long n_round = (n + stride - 1) / stride * stride;  // every thread of a warp runs every iteration
+  bool nan = false;
   for (long long i = blockIdx.x * static_cast<long long>(RED_T) + threadIdx.x; i < n_round; i += stride) {
     bool ok = i < n;
     unsigned long long u = ok ? pc_dkey(x[i]) : 0ull;
+    nan |= ok && (u > KEY_PINF || u < KEY_NINF);
     ok = ok && (u & mask) == prefix;
     hist_add(h, ok, static_cast<uint32_t>((u >> shift) & 255u));
   }
+  if (shift == 56 && __any_sync(0xffffffffu, nan) && (threadIdx.x & 31) == 0) s->nan = 1;
   __syncthreads();
   if (h[threadIdx.x]) atomicAdd(&hist[threadIdx.x], h[threadIdx.x]);
 }
@@ -654,9 +662,13 @@ __global__ void __launch_bounds__(RED_T) sel_succ_kernel(const double* __restric
   }
 }
 
-// numpy.median: the middle order statistic, or the mean (a + b) / 2 of the two middle ones
+// numpy.median: the middle order statistic, or the mean (a + b) / 2 of the two middle ones; NaN if any element is NaN
 __global__ void sel_final_kernel(const SelState* s, int n, double* out) {
   if (threadIdx.x != 0) return;
+  if (s->nan) {
+    *out = NAN;
+    return;
+  }
   const double a = pc_dkey_inv(s->prefix);
   if (n & 1) {
     *out = a;

@@ -102,9 +102,14 @@ def completion(gt_points, rec_points, gt_normals=None, rec_normals=None, device=
     return _metric(rec_points, gt_points, rec_normals, gt_normals, device, gather_ref=False)
 
 
+EXACT_F32_SUM = 1 << 24  # numpy's float32 sum of n ones and zeros is exact (every partial sum an integer <= 2^24)
+
+
 def completion_ratio(gt_points, rec_points, dist_th=0.05):
-    """np.mean((dist < dist_th).astype(np.float32)) over the ground-truth points (recon_metric.py:14-18).  numpy sums
-    the float32 ones exactly up to 2^24 points; so does this (count / n in float32)."""
+    """np.mean((dist < dist_th).astype(np.float32)) over the ground-truth points (recon_metric.py:14-18).  Up to 2^24
+    points numpy's float32 sum is the exact count, so this is float32(count) / float32(n) from a device count.  Past
+    that, numpy's pairwise float32 partial sums round and its result depends on where the ones lie; the distances are
+    copied to the host and the reference's own expression is evaluated on them."""
     dev = _device((gt_points, rec_points), None)
     r, q = _upload(rec_points, dev, "reconstructed points"), _upload(gt_points, dev, "ground-truth points")
     _check_finite(("reconstructed points", r), ("ground-truth points", q))
@@ -112,6 +117,8 @@ def completion_ratio(gt_points, rec_points, dist_th=0.05):
     if n == 0:
         return np.float32(np.nan)
     dist, _ = _nn(r, q)
+    if n > EXACT_F32_SUM:
+        return np.mean((dist.cpu().numpy() < dist_th).astype(np.float32))
     count = int(ops.f64_count_below(dist, float(dist_th)).item())
     return np.float32(count) / np.float32(n)
 
