@@ -455,6 +455,8 @@ int f3r_ingest_rgb8(const uint8_t* src, int32_t h, int32_t w, int32_t oh, int32_
                     int32_t hks, int32_t h_span_max, const int32_t* vb, const int32_t* vk, int32_t vks, uint8_t* tmp,
                     int32_t left, int32_t top, int32_t cw, int32_t ch, float* out, void* stream) {
   if (!src || !out) return fail("f3r_ingest_rgb8: null operand");
+  // the horizontal pass loads the source as 32-bit words counted from src (checked before the shape)
+  if (reinterpret_cast<uintptr_t>(src) & 3) return fail("f3r_ingest_rgb8: src not 4-byte aligned");
   if (h <= 0 || w <= 0 || oh <= 0 || ow <= 0 || cw <= 0 || ch <= 0) return fail("f3r_ingest_rgb8: bad shape");
   if (left < 0 || top < 0 || left + cw > ow || top + ch > oh) return fail("f3r_ingest_rgb8: crop box outside the resized image");
   if ((ow != w) != (hk != nullptr) || (oh != h) != (vk != nullptr))

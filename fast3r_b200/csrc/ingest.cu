@@ -86,6 +86,31 @@ resize_h_kernel(const uint8_t* __restrict__ src, int h, int w, uint8_t* __restri
   }
 }
 
+// ---- horizontal pass without shared memory, for geometries whose taps and spans exceed ING_SMEM_CAP (panoramas wider
+// than ~32 000 px at size 512): one thread per output pixel reads its taps and source bytes straight from global memory.
+// Same integer sums as resize_h_kernel, so the same bytes.
+constexpr size_t ING_SMEM_CAP = 200 * 1024;
+__global__ void __launch_bounds__(256)
+resize_h_direct_kernel(const uint8_t* __restrict__ src, int h, int w, uint8_t* __restrict__ dst, int ow,
+                       const int32_t* __restrict__ bounds, const int32_t* __restrict__ kk, int ksize) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= ow) return;
+  const int xmin = __ldg(bounds + 2 * x), n = __ldg(bounds + 2 * x + 1);
+  const int32_t* k = kk + static_cast<size_t>(x) * ksize;
+  for (int y = blockIdx.y; y < h; y += gridDim.y) {  // grid.y is capped at 65535 rows
+    const uint8_t* px = src + (static_cast<size_t>(y) * w + xmin) * 3;
+    int a0 = 1 << (ING_PREC - 1), a1 = a0, a2 = a0;
+    for (int t = 0; t < n; ++t) {
+      const int kv = __ldg(k + t);
+      a0 += static_cast<int>(__ldg(px + 3 * t + 0)) * kv;
+      a1 += static_cast<int>(__ldg(px + 3 * t + 1)) * kv;
+      a2 += static_cast<int>(__ldg(px + 3 * t + 2)) * kv;
+    }
+    uint8_t* o = dst + (static_cast<size_t>(y) * ow + x) * 3;
+    o[0] = ing_clip8(a0); o[1] = ing_clip8(a1); o[2] = ing_clip8(a2);
+  }
+}
+
 // ---- vertical pass fused with the center crop and ToTensor + Normalize:
 // mid [mh][mw][3] u8 (rows resampled to oh with the given taps, or used as they are when vk == nullptr)
 //   -> out fp32 [3][ch][cw],  out = ((v / 255) - 0.5) / 0.5  in fp32 like torchvision.
@@ -120,16 +145,26 @@ resize_v_crop_norm_kernel(const uint8_t* __restrict__ mid, int mw, const int32_t
   out[2 * plane + o] = __fdiv_rn(__fsub_rn(__fdiv_rn(static_cast<float>(v2), 255.0f), 0.5f), 0.5f);
 }
 
+// dynamic shared memory of resize_h_kernel: taps [ksize][ING_COLS] + ING_ROWS source spans
+static size_t ingest_h_smem(int hks, int h_span_max) {
+  return static_cast<size_t>(hks) * ING_COLS * 4 + static_cast<size_t>(ING_ROWS) * (((h_span_max * 3 + 3) & ~3) + 4);
+}
+
 cudaError_t launch_ingest(const uint8_t* src, int h, int w, int oh, int ow, const int32_t* hb, const int32_t* hk, int hks,
                           int h_span_max, const int32_t* vb, const int32_t* vk, int vks, uint8_t* tmp, int left, int top,
                           int cw, int ch, float* out, cudaStream_t stream) {
   const uint8_t* mid = src;
   if (hk != nullptr) {
-    const size_t smem = static_cast<size_t>(hks) * ING_COLS * 4 + static_cast<size_t>(ING_ROWS) * (((h_span_max * 3 + 3) & ~3) + 4);
-    if (smem > 200 * 1024) return cudaErrorInvalidValue;
-    dim3 grid((ow + ING_COLS - 1) / ING_COLS, (h + ING_ROWS_PER_BLOCK - 1) / ING_ROWS_PER_BLOCK);
-    const cudaError_t e = launch(resize_h_kernel, grid, ING_COLS * ING_ROWS, smem, stream, false, src, h, w, tmp, ow, hb, hk,
-                                 hks, h_span_max);
+    const size_t smem = ingest_h_smem(hks, h_span_max);
+    cudaError_t e;
+    if (smem <= ING_SMEM_CAP) {
+      dim3 grid((ow + ING_COLS - 1) / ING_COLS, (h + ING_ROWS_PER_BLOCK - 1) / ING_ROWS_PER_BLOCK);
+      e = launch(resize_h_kernel, grid, ING_COLS * ING_ROWS, smem, stream, false, src, h, w, tmp, ow, hb, hk, hks,
+                 h_span_max);
+    } else {
+      e = launch(resize_h_direct_kernel, dim3((ow + 255) / 256, h < 65535 ? h : 65535), 256, 0, stream, false, src, h, w,
+                 tmp, ow, hb, hk, hks);
+    }
     if (e != cudaSuccess) return e;
     mid = tmp;
   }

@@ -53,7 +53,8 @@ inline bool build_huff(const uint8_t* counts, const uint8_t* vals, int nvals, Hu
       }
     }
     t->maxcode[len] = counts[len - 1] ? code - 1 : -1;
-    if (code > (1 << len)) return false;  // over-subscribed
+    // over-subscribed, or a code of all ones: libjpeg (jpeg_make_d_derived_tbl) rejects code >= 2^len after each length
+    if (code >= (1 << len)) return false;
     code <<= 1;
   }
   t->maxcode[0] = -1;
@@ -137,6 +138,9 @@ inline int parse(const uint8_t* d, size_t n, Header* h) {
           for (int i = 0; i < 16; ++i) total += s[q + 1 + i];
           if (tc > 1 || total > 256 || q + 17 + total > sl) return finish(h, kMalformed, "bad DHT");
           if (th > 1) return finish(h, kUnsupported, "Huffman table slot above 1");
+          // libjpeg rejects a DC table with a symbol above 15 whether or not the scan codes it
+          for (int i = 0; i < total && tc == 0; ++i)
+            if (s[q + 17 + i] > 15) return finish(h, kMalformed, "DC Huffman symbol above 15");
           HuffTable* t = tc ? &h->ac[th] : &h->dc[th];
           if (!build_huff(s + q + 1, s + q + 17, total, t)) return finish(h, kMalformed, "bad Huffman table");
           (tc ? h->ac_set : h->dc_set)[th] = true;

@@ -65,12 +65,28 @@ def _tables(in_size: int, out_size: int, filt: int, device):
     return _TABLES[key]
 
 
+def _need_cuda(device, what: str):
+    """Raises unless `device` is a CUDA device: the library has no CPU path."""
+    if torch.device(device).type != "cuda":
+        raise RuntimeError(what)
+
+
+def _h2d(arr: np.ndarray, device) -> torch.Tensor:
+    """Copies a host uint8 array to `device` through a pinned staging buffer (asynchronous on the current stream)."""
+    host = torch.empty(arr.shape, dtype=torch.uint8, pin_memory=True)
+    host.numpy()[...] = arr
+    return host.to(device, non_blocking=True)
+
+
 def ingest_rgb8(img_u8: torch.Tensor, size: int = 512, square_ok: bool = False, out: torch.Tensor = None):
     """img_u8: CUDA uint8 (h, w, 3) RGB.  Returns (fp32 (3, H, W) in [-1, 1], (H, W)): resize + crop + normalise of
     load_images()."""
-    if not img_u8.is_cuda or img_u8.dtype != torch.uint8 or img_u8.dim() != 3 or img_u8.shape[2] != 3:
+    if img_u8.dtype != torch.uint8 or img_u8.dim() != 3 or img_u8.shape[2] != 3:
         raise RuntimeError("ingest_rgb8 needs a CUDA uint8 (h, w, 3) tensor (there is no CPU path)")
+    _need_cuda(img_u8.device, "ingest_rgb8 needs a CUDA uint8 (h, w, 3) tensor (there is no CPU path)")
     img_u8 = img_u8.contiguous()
+    if img_u8.data_ptr() % 4:  # e.g. a row slice of an image whose width is not a multiple of 4; the library needs 4
+        img_u8 = img_u8.clone()
     h1, w1, _ = img_u8.shape
     if size == 224:
         nw, nh, filt = resize_plan(w1, h1, round(size * max(w1 / h1, h1 / w1)))
@@ -164,9 +180,7 @@ def _decode_jpeg_async(data, probe: JpegProbe, orientation: int, rotate_clockwis
     """Enqueues the device decode of a supported JPEG on the current stream.  Returns the uint8 (h, w, 3) image and a
     device int32 status (0: decoded; non-zero: the entropy-coded data is inconsistent and the image is undefined)."""
     buf = np.frombuffer(data, np.uint8)
-    host = torch.empty(len(buf), dtype=torch.uint8, pin_memory=True)
-    host.numpy()[:] = buf
-    dev = host.to(device, non_blocking=True)
+    dev = _h2d(buf, device)
     oh, ow, left, top = _store_geometry(probe.width, probe.height, orientation, rotate_clockwise_90, crop_to_landscape)
     out = torch.empty(oh, ow, 3, dtype=torch.uint8, device=device)
     status = torch.zeros(1, dtype=torch.int32, device=device)
@@ -185,8 +199,7 @@ def decode_jpeg(data, rotate_clockwise_90: bool = False, crop_to_landscape: bool
     4:3 crop) returns for the same file.  Raises ValueError for a file the GPU does not decode (progressive, CMYK,
     non-JPEG, ...; see probe_jpeg) and RuntimeError when the entropy-coded data is inconsistent.  Synchronises."""
     device = torch.device(device)
-    if device.type != "cuda":
-        raise RuntimeError("decode_jpeg decodes on a CUDA device (there is no CPU path)")
+    _need_cuda(device, "decode_jpeg decodes on a CUDA device (there is no CPU path)")
     probe = probe_jpeg(data)
     if probe.status != L.JPEG_SUPPORTED:
         raise ValueError(f"not a JPEG the GPU decodes: {probe.why}")
@@ -226,9 +239,8 @@ def load_images(folder_or_list, size, square_ok=False, verbose=True, rotate_cloc
     else:
         raise ValueError(f"bad {folder_or_list=} ({type(folder_or_list)})")
     device = torch.device(device)
-    if device.type != "cuda":
-        raise RuntimeError("fast3r_b200.ingest.load_images produces CUDA views (no CPU path); use the reference's "
-                           "load_images for host tensors")
+    _need_cuda(device, "fast3r_b200.ingest.load_images produces CUDA views (no CPU path); use the reference's "
+                       "load_images for host tensors")
     L.load()
     exts = (".jpg", ".jpeg", ".png", ".heic", ".heif")
     paths = [os.path.join(root, p) for p in folder_content if p.lower().endswith(exts)]
@@ -236,7 +248,7 @@ def load_images(folder_or_list, size, square_ok=False, verbose=True, rotate_cloc
     imgs = []
 
     def upload(arr):
-        return torch.from_numpy(np.ascontiguousarray(arr)).pin_memory().to(device, non_blocking=True)
+        return _h2d(np.ascontiguousarray(arr), device)
 
     with ThreadPoolExecutor(max_workers=num_threads or min(32, os.cpu_count() or 4)) as pool:
         for path, (data, probe, payload) in zip(paths, pool.map(

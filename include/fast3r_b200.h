@@ -158,7 +158,8 @@ int f3r_cast_f16(const float* in, void* out, size_t count, void* stream);
  * one dimension: bounds [out_size][2] = (first tap, count), kk [out_size][f3r_resample_ksize()] fixed-point weights, and
  * returns the widest source span of 64 consecutive outputs (h_span_max below; < 0 on error).  f3r_ingest_rgb8 takes DEVICE
  * copies of the tables (NULL for a dimension that keeps its size), a device scratch tmp [h][ow][3] (when ow != w) and
- * writes the crop box (left, top, cw, ch) of the resized image as fp32 [3][ch][cw] in [-1, 1]. */
+ * writes the crop box (left, top, cw, ch) of the resized image as fp32 [3][ch][cw] in [-1, 1].  src must be 4-byte
+ * aligned (refused before any CUDA call otherwise). */
 int f3r_resample_ksize(int32_t in_size, int32_t out_size, int32_t filter);
 int f3r_resample_coeffs(int32_t in_size, int32_t out_size, int32_t filter, int32_t* bounds, int32_t* kk);
 int f3r_ingest_rgb8(const uint8_t* src, int32_t h, int32_t w, int32_t oh, int32_t ow, const int32_t* hb, const int32_t* hk,
