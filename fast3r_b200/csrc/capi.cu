@@ -606,6 +606,75 @@ int f3r_f64_count_below(const double* x, int32_t n, const double* th, uint64_t* 
                                            static_cast<cudaStream_t>(stream)), "f3r_f64_count_below");
 }
 
+// ---------------------------------------------------------------- camera poses
+size_t f3r_pnp_gather_workspace(int32_t views, int32_t h, int32_t w) {
+  return views > 0 && h > 0 && w > 0 && static_cast<long long>(h) * w <= (1 << 30)
+             ? f3r::pnp_gather_workspace(views, h * w) : 0;
+}
+
+int f3r_pnp_gather(const float* pts, const float* conf, const uint8_t* mask, int32_t views, int32_t h, int32_t w,
+                   float* out_pts, float* out_pix, int32_t* counts, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!pts || !out_pts || !out_pix || !counts || !workspace) return fail("f3r_pnp_gather: null operand");
+  if ((conf != nullptr) == (mask != nullptr)) return fail("f3r_pnp_gather: give exactly one of conf and mask");
+  if (views <= 0 || views > 65535 || h <= 0 || w <= 0 || static_cast<long long>(h) * w > (1 << 30))
+    return fail("f3r_pnp_gather: bad shape views=%d h=%d w=%d", views, h, w);
+  if (workspace_bytes < f3r::pnp_gather_workspace(views, h * w)) return fail("f3r_pnp_gather: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 3) return fail("f3r_pnp_gather: workspace not 4-byte aligned");
+  return check(f3r::launch_pnp_gather(pts, conf, mask, views, h, w, out_pts, out_pix, counts, workspace,
+                                      static_cast<cudaStream_t>(stream)), "f3r_pnp_gather");
+}
+
+// the host tables of f3r_pnp_score / f3r_pnp_inliers; returns the largest view count or -1 (after fail()) if invalid
+static int pnp_tables(const char* what, const int64_t* offsets, const int32_t* view_counts, int32_t views,
+                      const f3r_pnp_hyp* hyps, int32_t nh, float thr) {
+  if (!offsets || !view_counts || !hyps) return fail("%s: null table", what), -1;
+  if (views <= 0 || nh <= 0) return fail("%s: bad sizes views=%d nh=%d", what, views, nh), -1;
+  if (!(thr >= 0.f && thr <= 3.4028234663852886e38f)) return fail("%s: threshold %g is not finite and >= 0", what, thr), -1;
+  int max_count = 0;
+  for (int v = 0; v < views; ++v) {
+    if (view_counts[v] < 0 || offsets[v] < 0) return fail("%s: view %d has offset %lld and count %d", what, v,
+                                                            static_cast<long long>(offsets[v]), view_counts[v]), -1;
+    max_count = view_counts[v] > max_count ? view_counts[v] : max_count;
+  }
+  for (int r = 0; r < nh; ++r)
+    if (hyps[r].view < 0 || hyps[r].view >= views)
+      return fail("%s: hypothesis %d names view %d of %d", what, r, hyps[r].view, views), -1;
+  return max_count;
+}
+
+size_t f3r_pnp_score_workspace(int32_t views, int32_t nh) {
+  return views > 0 && nh > 0 ? f3r::pnp_score_workspace(views, nh) : 0;
+}
+
+int f3r_pnp_score(const float* pts, const float* pix, const int64_t* offsets, const int32_t* view_counts, int32_t views,
+                  const f3r_pnp_hyp* hyps, int32_t nh, float thr, int32_t* counts, void* workspace, size_t workspace_bytes,
+                  void* stream) {
+  if (!pts || !pix || !counts || !workspace) return fail("f3r_pnp_score: null operand");
+  if (pnp_tables("f3r_pnp_score", offsets, view_counts, views, hyps, nh, thr) < 0) return 1;
+  if (workspace_bytes < f3r::pnp_score_workspace(views, nh)) return fail("f3r_pnp_score: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("f3r_pnp_score: workspace not 256-byte aligned");
+  return check(f3r::launch_pnp_score(pts, pix, reinterpret_cast<const long long*>(offsets), view_counts, views, hyps, nh,
+                                     thr, counts, workspace, static_cast<cudaStream_t>(stream)), "f3r_pnp_score");
+}
+
+size_t f3r_pnp_inliers_workspace(int32_t nh, int32_t max_count) {
+  return nh > 0 && max_count >= 0 ? f3r::pnp_inliers_workspace(nh, max_count) : 0;
+}
+
+int f3r_pnp_inliers(const float* pts, const float* pix, const int64_t* offsets, const int32_t* view_counts, int32_t views,
+                    const f3r_pnp_hyp* hyps, int32_t nh, float thr, float* out_pts, float* out_pix, int32_t* out_counts,
+                    void* workspace, size_t workspace_bytes, void* stream) {
+  if (!pts || !pix || !out_pts || !out_pix || !out_counts || !workspace) return fail("f3r_pnp_inliers: null operand");
+  const int max_count = pnp_tables("f3r_pnp_inliers", offsets, view_counts, views, hyps, nh, thr);
+  if (max_count < 0) return 1;
+  if (nh > 65535) return fail("f3r_pnp_inliers: %d rows (at most 65535)", nh);
+  if (workspace_bytes < f3r::pnp_inliers_workspace(nh, max_count)) return fail("f3r_pnp_inliers: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("f3r_pnp_inliers: workspace not 256-byte aligned");
+  return check(f3r::launch_pnp_inliers(pts, pix, reinterpret_cast<const long long*>(offsets), view_counts, hyps, nh, thr,
+                                       out_pts, out_pix, out_counts, workspace, static_cast<cudaStream_t>(stream)),
+               "f3r_pnp_inliers");
+}
+
 int f3r_cast_bf16(const float* in, void* out, size_t count, void* stream) {
   if (!in || !out) return fail("f3r_cast_bf16: null operand");
   return check(f3r::launch_cast_bf16(in, out, count, static_cast<cudaStream_t>(stream)), "f3r_cast_bf16");

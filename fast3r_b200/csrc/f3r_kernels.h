@@ -186,4 +186,16 @@ cudaError_t launch_f64_median(const double* x, int n, double* out, void* workspa
 cudaError_t launch_f64_count_below(const double* x, int n, const double* th, unsigned long long* count,
                                    cudaStream_t stream);
 
+// camera poses (pose.cu); offsets, counts_in and hyps are host arrays
+size_t pnp_gather_workspace(int views, int n);
+cudaError_t launch_pnp_gather(const float* pts, const float* conf, const uint8_t* mask, int views, int h, int w,
+                              float* out_pts, float* out_pix, int* counts, void* workspace, cudaStream_t stream);
+size_t pnp_score_workspace(int views, int nh);
+cudaError_t launch_pnp_score(const float* pts, const float* pix, const long long* offsets, const int* counts_in, int views,
+                             const f3r_pnp_hyp* hyps, int nh, float thr, int* counts, void* workspace, cudaStream_t stream);
+size_t pnp_inliers_workspace(int nh, int max_count);
+cudaError_t launch_pnp_inliers(const float* pts, const float* pix, const long long* offsets, const int* counts_in,
+                               const f3r_pnp_hyp* hyps, int nh, float thr, float* out_pts, float* out_pix, int* counts,
+                               void* workspace, cudaStream_t stream);
+
 }  // namespace f3r

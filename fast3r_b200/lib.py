@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfast3r_b200.so")
 
@@ -43,6 +45,11 @@ ABI_VERSION = 3
 
 
 JPEG_SUPPORTED, JPEG_UNSUPPORTED, JPEG_MALFORMED = range(3)
+
+
+# one row of the hypothesis table of f3r_pnp_score / f3r_pnp_inliers (f3r_pnp_hyp), as a numpy record
+PNP_HYP = np.dtype([("r", "<f8", (9,)), ("t", "<f8", (3,)), ("fx", "<f8"), ("fy", "<f8"), ("cx", "<f8"), ("cy", "<f8"),
+                    ("view", "<i4"), ("reserved", "<i4")])
 
 
 class JpegInfo(C.Structure):
@@ -106,6 +113,12 @@ _API = {
     "f3r_f64_mean": (C.c_int, [_P, _I32, _P, _P, _SIZE, _P]),
     "f3r_f64_median": (C.c_int, [_P, _I32, _P, _P, _SIZE, _P]),
     "f3r_f64_count_below": (C.c_int, [_P, _I32, _P, _P, _P]),
+    "f3r_pnp_gather_workspace": (_SIZE, [_I32, _I32, _I32]),
+    "f3r_pnp_gather": (C.c_int, [_P, _P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _SIZE, _P]),
+    "f3r_pnp_score_workspace": (_SIZE, [_I32, _I32]),
+    "f3r_pnp_score": (C.c_int, [_P, _P, _P, _P, _I32, _P, _I32, _F32, _P, _P, _SIZE, _P]),
+    "f3r_pnp_inliers_workspace": (_SIZE, [_I32, _I32]),
+    "f3r_pnp_inliers": (C.c_int, [_P, _P, _P, _P, _I32, _P, _I32, _F32, _P, _P, _P, _P, _SIZE, _P]),
 }
 EXPORTS = list(_API)
 

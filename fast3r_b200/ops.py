@@ -5,6 +5,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import Optional
 
+import numpy as np
 import torch
 
 from . import lib as L
@@ -408,6 +409,71 @@ def focal_weiszfeld(pts: torch.Tensor, conf: Optional[torch.Tensor] = None, thr:
     _call("f3r_focal_weiszfeld", pts, _ptr(pts), _ptr(conf), _ptr(thr), _ptr(pp), views, h, w, int(iters), _ptr(focal),
           _ptr(ws), nbytes)
     return focal
+
+
+# ------------------------------------------------------------------ camera poses (csrc/pose.cu)
+def pnp_gather(pts: torch.Tensor, conf: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None):
+    """pts fp32 [views, H, W, 3] and either conf fp32 [views, H, W] (selects conf > 1) or mask uint8 [views, H, W].
+    Returns (points fp32 [views, H W, 3], pixels fp32 [views, H W, 2], counts int32 [views]): the first counts[v] rows
+    of view v are its selected pixels in raster order with their pixel_grid coordinates (x, y)."""
+    _chk(pts, F32, "pts")
+    views, h, w = pts.shape[0], pts.shape[1], pts.shape[2]
+    assert pts.shape == (views, h, w, 3) and (conf is None) != (mask is None)
+    if conf is not None:
+        _chk(conf, F32, "conf")
+        assert conf.shape == (views, h, w)
+    else:
+        _chk(mask, torch.uint8, "mask")
+        assert mask.shape == (views, h, w)
+    nbytes = L.load().f3r_pnp_gather_workspace(views, h, w)
+    ws = _scratch(max(nbytes, 4), pts.device)
+    out_pts = torch.empty(views, h * w, 3, dtype=F32, device=pts.device)
+    out_pix = torch.empty(views, h * w, 2, dtype=F32, device=pts.device)
+    counts = torch.empty(views, dtype=torch.int32, device=pts.device)
+    _call("f3r_pnp_gather", pts, _ptr(pts), _ptr(conf), _ptr(mask), views, h, w, _ptr(out_pts), _ptr(out_pix), _ptr(counts),
+          _ptr(ws), nbytes)
+    return out_pts, out_pix, counts
+
+
+def _pnp_tables(pts, pix, offsets, view_counts, hyps):
+    _chk(pts, F32, "pts"); _chk(pix, F32, "pix")
+    assert pts.dim() == 2 and pts.shape[1] == 3 and pix.shape == (pts.shape[0], 2)
+    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+    view_counts = np.ascontiguousarray(view_counts, dtype=np.int32)
+    hyps = np.ascontiguousarray(hyps, dtype=L.PNP_HYP)
+    assert offsets.shape == view_counts.shape and offsets.ndim == 1 and hyps.ndim == 1
+    if len(offsets) and int((offsets + view_counts).max()) > pts.shape[0]:
+        raise ValueError("pnp: a view reaches past the points")
+    return offsets, view_counts, hyps
+
+
+def pnp_score(pts: torch.Tensor, pix: torch.Tensor, offsets, view_counts, hyps, thr: float) -> torch.Tensor:
+    """Inlier counts int32 [nh] (device) of the hypothesis table `hyps` (host records of lib.PNP_HYP): row r counts the
+    points of view hyps[r]["view"] = pts/pix rows [offsets[v], offsets[v] + view_counts[v]) (host int arrays) whose
+    reprojection error is <= thr (OpenCV's arithmetic, pose_math.h)."""
+    offsets, view_counts, hyps = _pnp_tables(pts, pix, offsets, view_counts, hyps)
+    nbytes = L.load().f3r_pnp_score_workspace(len(offsets), len(hyps))
+    ws = _scratch(nbytes, pts.device)
+    counts = torch.empty(len(hyps), dtype=torch.int32, device=pts.device)
+    _call("f3r_pnp_score", pts, _ptr(pts), _ptr(pix), offsets.ctypes.data, view_counts.ctypes.data, len(offsets),
+          hyps.ctypes.data, len(hyps), float(thr), _ptr(counts), _ptr(ws), nbytes)
+    return counts
+
+
+def pnp_inliers(pts: torch.Tensor, pix: torch.Tensor, offsets, view_counts, hyps, thr: float):
+    """The inliers of each row r of `hyps` among the points of its view (the rule of pnp_score), in index order.  Returns
+    (points fp32 [m, 3], pixels fp32 [m, 2], counts int32 [nh]) on the device: row r's inliers are the first counts[r]
+    rows from slot sum_{s<r} view_counts[hyps[s]["view"]] on (m is the sum over all rows)."""
+    offsets, view_counts, hyps = _pnp_tables(pts, pix, offsets, view_counts, hyps)
+    m = int(view_counts[hyps["view"]].astype(np.int64).sum())
+    nbytes = L.load().f3r_pnp_inliers_workspace(len(hyps), int(view_counts.max()))
+    ws = _scratch(nbytes, pts.device)
+    out_pts = torch.empty(max(m, 1), 3, dtype=F32, device=pts.device)
+    out_pix = torch.empty(max(m, 1), 2, dtype=F32, device=pts.device)
+    counts = torch.empty(len(hyps), dtype=torch.int32, device=pts.device)
+    _call("f3r_pnp_inliers", pts, _ptr(pts), _ptr(pix), offsets.ctypes.data, view_counts.ctypes.data, len(offsets),
+          hyps.ctypes.data, len(hyps), float(thr), _ptr(out_pts), _ptr(out_pix), _ptr(counts), _ptr(ws), nbytes)
+    return out_pts[:m], out_pix[:m], counts
 
 
 # ------------------------------------------------------------------ reconstruction metrics (csrc/pointcloud.cu)

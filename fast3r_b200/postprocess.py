@@ -13,8 +13,10 @@ Same names, arguments and results as the reference:
 * ``evaluate_reconstruction(views, preds, ...)`` - MultiViewDUSt3RLitModule.evaluate_reconstruction
   (multiview_dust3r_module.py:551-735): registration, normals and the metrics of fast3r_b200.recon_metric per batch item.
 
-NOT here (documented in DESIGN.md §1): fast_pnp / cv2.solvePnPRansac (cloud_opt/init_im_poses.py:300-350) and the
-"median" focal mode.  Tensors may live on the CPU (what ``inference()`` returns) or on a CUDA device; CPU inputs are
+* ``fast_pnp``, ``estimate_cam_pose_one_sample`` and ``estimate_camera_poses`` - the camera poses, re-exported from
+  fast3r_b200.poses (RANSAC scoring on the GPU, bit-identical to cv2.solvePnPRansac).
+
+NOT here (documented in DESIGN.md §1): the "median" focal mode.  Tensors may live on the CPU (what ``inference()`` returns) or on a CUDA device; CPU inputs are
 copied to ``device`` (default cuda:0) and the results copied back, so the function is a drop-in either way.  There is
 no CPU implementation: without the CUDA library this raises.
 """
@@ -95,6 +97,9 @@ def estimate_focal(pts3d_i: torch.Tensor, conf_i: torch.Tensor, pp: Optional[tor
     thr = ops.conf_quantile(conf.reshape(b, h * w), float(min_conf_thr_percentile) / 100.0)
     ppt = None if pp is None else _f32(torch.as_tensor(pp), dev).reshape(b, 2)
     return float(ops.focal_weiszfeld(pts, conf, thr, ppt, iters=100)[0])
+
+
+from .poses import estimate_cam_pose_one_sample, estimate_camera_poses, fast_pnp  # noqa: E402,F401
 
 
 def estimate_focal_knowing_depth(pts3d: torch.Tensor, pp: torch.Tensor, focal_mode: str = "weiszfeld", device=None) -> torch.Tensor:

@@ -275,6 +275,42 @@ int f3r_f64_mean(const double* x, int32_t n, double* out, void* workspace, size_
 int f3r_f64_median(const double* x, int32_t n, double* out, void* workspace, size_t workspace_bytes, void* stream);
 int f3r_f64_count_below(const double* x, int32_t n, const double* th, uint64_t* count, void* stream);
 
+/* ---- camera poses: the per-point work of cv2.solvePnPRansac(..., flags=SOLVEPNP_SQPNP) as fast_pnp calls it
+ * (fast3r/dust3r/cloud_opt/init_im_poses.py:300-350), exact with respect to OpenCV's classic RANSAC.  The host draws
+ * the samples, solves the EPnP hypotheses, keeps the books and refits (fast3r_b200/poses.py).
+ *
+ * f3r_pnp_gather: per view v of n = h w pixels, the pixels with conf > 1 (conf given, mask NULL) or mask != 0 (mask
+ *   given, conf NULL) in raster order, as numpy's boolean indexing orders them: out_pts [views][n][3] gets the points,
+ *   out_pix [views][n][2] their pixel_grid coordinates (x, y), both from slot v n on; counts [views] (int32) how many.
+ *   workspace: f3r_pnp_gather_workspace(views, h, w) bytes, 4-byte aligned.
+ * f3r_pnp_score: counts[r] = the number of points of view hyps[r].view whose error under hypothesis r is
+ *   <= (float)(thr * thr): OpenCV's projectPoints with zero distortion in double, stored as float, then the float
+ *   |pixel - projection|^2 (fast3r_b200/csrc/pose_math.h).  Points and pixels are DEVICE arrays (pts [.][3], pix [.][2]);
+ *   view v is [offsets[v], offsets[v] + view_counts[v]) of them.  offsets, view_counts and hyps are HOST arrays.  Rows
+ *   of one view that follow each other share their reads of the points.  workspace: f3r_pnp_score_workspace(views, nh)
+ *   bytes, 256-byte aligned.
+ * f3r_pnp_inliers: for every row r the points and pixels of view hyps[r].view that are inliers of hypothesis r (the
+ *   rule of f3r_pnp_score), in index order, into out_pts / out_pix from slot sum_{s<r} view_counts[hyps[s].view] on;
+ *   out_counts [nh] (int32, device) how many.  workspace: f3r_pnp_inliers_workspace(nh, max view_counts) bytes, 256-byte
+ *   aligned. */
+typedef struct f3r_pnp_hyp {
+  double r[9];                /* rotation, row-major: cv2.Rodrigues of the hypothesis' rvec */
+  double t[3];
+  double fx, fy, cx, cy;      /* the camera matrix as double */
+  int32_t view, reserved;
+} f3r_pnp_hyp;
+size_t f3r_pnp_gather_workspace(int32_t views, int32_t h, int32_t w);
+int f3r_pnp_gather(const float* pts, const float* conf, const uint8_t* mask, int32_t views, int32_t h, int32_t w,
+                   float* out_pts, float* out_pix, int32_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+size_t f3r_pnp_score_workspace(int32_t views, int32_t nh);
+int f3r_pnp_score(const float* pts, const float* pix, const int64_t* offsets, const int32_t* view_counts, int32_t views,
+                  const f3r_pnp_hyp* hyps, int32_t nh, float thr, int32_t* counts, void* workspace, size_t workspace_bytes,
+                  void* stream);
+size_t f3r_pnp_inliers_workspace(int32_t nh, int32_t max_count);
+int f3r_pnp_inliers(const float* pts, const float* pix, const int64_t* offsets, const int32_t* view_counts, int32_t views,
+                    const f3r_pnp_hyp* hyps, int32_t nh, float thr, float* out_pts, float* out_pix, int32_t* out_counts,
+                    void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
