@@ -675,6 +675,86 @@ int f3r_pnp_inliers(const float* pts, const float* pix, const int64_t* offsets, 
                "f3r_pnp_inliers");
 }
 
+// ---------------------------------------------------------------- viewer scene
+static bool sky_shape_ok(int32_t frames, int32_t h, int32_t w) {
+  return frames > 0 && h > 0 && w > 0 && static_cast<long long>(frames) * h * w < (1ll << 31);
+}
+
+size_t f3r_sky_mask_workspace(int32_t frames, int32_t h, int32_t w) {
+  return sky_shape_ok(frames, h, w) ? f3r::sky_mask_workspace(frames, h, w) : 0;
+}
+
+int f3r_sky_mask(const float* img, int32_t frames, int32_t h, int32_t w, int32_t upper_rows, int32_t min_sky,
+                 int8_t* not_sky, int32_t* not_sky_count, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!img || !not_sky || !not_sky_count || !workspace) return fail("f3r_sky_mask: null operand");
+  if (!sky_shape_ok(frames, h, w)) return fail("f3r_sky_mask: bad shape frames=%d h=%d w=%d", frames, h, w);
+  if (workspace_bytes < f3r::sky_mask_workspace(frames, h, w)) return fail("f3r_sky_mask: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("f3r_sky_mask: workspace not 256-byte aligned");
+  return check(f3r::launch_sky_mask(img, frames, h, w, upper_rows, min_sky, not_sky, not_sky_count, workspace,
+                                    static_cast<cudaStream_t>(stream)), "f3r_sky_mask");
+}
+
+size_t f3r_scene_sort_workspace(int32_t n) { return n > 0 ? f3r::scene_sort_workspace(n) : 0; }
+
+int f3r_scene_sort(const float* conf, const float* pts, const float* img, const int8_t* not_sky, const int64_t* offsets,
+                   int32_t frames, int32_t n, float* out_pts, uint8_t* out_rgb, int8_t* out_not_sky, float* max_conf,
+                   void* workspace, size_t workspace_bytes, void* stream) {
+  if (!conf || !pts || !img || !not_sky || !offsets || !out_pts || !out_rgb || !out_not_sky || !max_conf || !workspace)
+    return fail("f3r_scene_sort: null operand");
+  if (frames <= 0 || frames > (1 << 24) || n <= 0) return fail("f3r_scene_sort: bad sizes frames=%d n=%d", frames, n);
+  if (workspace_bytes < f3r::scene_sort_workspace(n)) return fail("f3r_scene_sort: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("f3r_scene_sort: workspace not 256-byte aligned");
+  return check(f3r::launch_scene_sort(conf, pts, img, not_sky, reinterpret_cast<const long long*>(offsets), frames, n,
+                                      out_pts, out_rgb, out_not_sky, max_conf, workspace,
+                                      static_cast<cudaStream_t>(stream)), "f3r_scene_sort");
+}
+
+static bool visible_sizes_ok(int32_t nseg, size_t max_len) {
+  return nseg > 0 && nseg <= 65535 && max_len > 0 && max_len < (1ull << 40);
+}
+
+size_t f3r_scene_visible_workspace(int32_t nseg, size_t max_len) {
+  return visible_sizes_ok(nseg, max_len) ? f3r::scene_visible_workspace(nseg, f3r::scene_visible_tiles(max_len)) : 0;
+}
+
+int f3r_scene_visible(const int64_t* segs, int32_t nseg, size_t max_len, const float* pts_g, const float* pts_l,
+                      const uint8_t* rgb_g, const uint8_t* rgb_l, const int8_t* not_sky_g, const int8_t* not_sky_l,
+                      int32_t mask_sky, uint64_t* total, float* out_pts, uint8_t* out_rgb, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+  if (!segs || !pts_g || !pts_l || !rgb_g || !rgb_l || !not_sky_g || !not_sky_l || !workspace)
+    return fail("f3r_scene_visible: null operand");
+  if ((total != nullptr) == (out_pts != nullptr) || (out_pts != nullptr) != (out_rgb != nullptr))
+    return fail("f3r_scene_visible: give total (counting) or out_pts and out_rgb (writing)");
+  if (!visible_sizes_ok(nseg, max_len)) return fail("f3r_scene_visible: bad sizes nseg=%d", nseg);
+  const int tiles = f3r::scene_visible_tiles(max_len);
+  if (tiles > (1 << 30)) return fail("f3r_scene_visible: segments too long");
+  if (workspace_bytes < f3r::scene_visible_workspace(nseg, tiles)) return fail("f3r_scene_visible: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("f3r_scene_visible: workspace not 256-byte aligned");
+  return check(f3r::launch_scene_visible(reinterpret_cast<const long long*>(segs), nseg, tiles, pts_g, pts_l, rgb_g,
+                                         rgb_l, not_sky_g, not_sky_l, mask_sky,
+                                         reinterpret_cast<unsigned long long*>(total), out_pts, out_rgb, workspace,
+                                         static_cast<cudaStream_t>(stream)), "f3r_scene_visible");
+}
+
+int f3r_ply_pack(const float* pts, const uint8_t* rgb, size_t n, uint8_t* out, void* stream) {
+  if (n && (!pts || !rgb || !out)) return fail("f3r_ply_pack: null operand");
+  return check(f3r::launch_ply_pack(pts, rgb, static_cast<long long>(n), out, static_cast<cudaStream_t>(stream)),
+               "f3r_ply_pack");
+}
+
+size_t f3r_extent_percentiles_workspace(void) { return f3r::percentile_workspace(); }
+
+int f3r_extent_percentiles(const float* pts, size_t n, size_t k0, size_t k1, float g0, float g1, float* out,
+                           void* workspace, size_t workspace_bytes, void* stream) {
+  if (!pts || !out || !workspace) return fail("f3r_extent_percentiles: null operand");
+  if (n == 0 || n >= (1ull << 32) || k0 >= n || k1 >= n) return fail("f3r_extent_percentiles: bad ranks");
+  if (workspace_bytes < f3r::percentile_workspace()) return fail("f3r_extent_percentiles: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 255) return fail("f3r_extent_percentiles: workspace not 256-byte aligned");
+  return check(f3r::launch_extent_percentiles(pts, static_cast<long long>(n), static_cast<long long>(k0),
+                                              static_cast<long long>(k1), g0, g1, out, workspace,
+                                              static_cast<cudaStream_t>(stream)), "f3r_extent_percentiles");
+}
+
 int f3r_cast_bf16(const float* in, void* out, size_t count, void* stream) {
   if (!in || !out) return fail("f3r_cast_bf16: null operand");
   return check(f3r::launch_cast_bf16(in, out, count, static_cast<cudaStream_t>(stream)), "f3r_cast_bf16");

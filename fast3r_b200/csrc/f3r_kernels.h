@@ -185,6 +185,11 @@ cudaError_t launch_f64_mean(const double* x, int n, double* out, void* workspace
 cudaError_t launch_f64_median(const double* x, int n, double* out, void* workspace, cudaStream_t stream);
 cudaError_t launch_f64_count_below(const double* x, int n, const double* th, unsigned long long* count,
                                    cudaStream_t stream);
+// the stable LSD radix sort of the index build: (keys, vals) by the low `bits` bits of the keys, ping-ponging between
+// buffer 0 and 1; *in_b tells (in and out) where the data is; hist: radix_sort_hist_bytes(n) bytes
+size_t radix_sort_hist_bytes(int n);
+cudaError_t launch_radix_sort(unsigned long long* keys[2], int* vals[2], int n, int bits, uint32_t* hist, int* in_b,
+                              cudaStream_t stream);
 
 // camera poses (pose.cu); offsets, counts_in and hyps are host arrays
 size_t pnp_gather_workspace(int views, int n);
@@ -197,5 +202,25 @@ size_t pnp_inliers_workspace(int nh, int max_count);
 cudaError_t launch_pnp_inliers(const float* pts, const float* pix, const long long* offsets, const int* counts_in,
                                const f3r_pnp_hyp* hyps, int nh, float thr, float* out_pts, float* out_pix, int* counts,
                                void* workspace, cudaStream_t stream);
+
+
+// viewer scene (scene.cu)
+size_t sky_mask_workspace(int frames, int h, int w);
+cudaError_t launch_sky_mask(const float* img, int frames, int h, int w, int upper, int min_sky, int8_t* not_sky,
+                            int* not_sky_count, void* workspace, cudaStream_t stream);
+size_t scene_sort_workspace(long long n);
+cudaError_t launch_scene_sort(const float* conf, const float* pts, const float* img, const int8_t* not_sky,
+                              const long long* off, int frames, int n, float* out_pts, uint8_t* out_rgb,
+                              int8_t* out_not_sky, float* max_conf, void* workspace, cudaStream_t stream);
+int scene_visible_tiles(long long max_len);
+size_t scene_visible_workspace(int nseg, int tiles);
+cudaError_t launch_scene_visible(const long long* segs, int nseg, int tiles, const float* pts_g, const float* pts_l,
+                                 const uint8_t* rgb_g, const uint8_t* rgb_l, const int8_t* ns_g, const int8_t* ns_l,
+                                 int mask_sky, unsigned long long* total, float* out_pts, uint8_t* out_rgb,
+                                 void* workspace, cudaStream_t stream);
+cudaError_t launch_ply_pack(const float* pts, const uint8_t* rgb, long long n, uint8_t* out, cudaStream_t stream);
+size_t percentile_workspace();
+cudaError_t launch_extent_percentiles(const float* pts, long long n, long long k0, long long k1, float g0, float g1,
+                                      float* out, void* workspace, cudaStream_t stream);
 
 }  // namespace f3r

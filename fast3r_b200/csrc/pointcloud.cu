@@ -718,6 +718,13 @@ size_t pc_index_workspace(int n) { return index_layout(n).total; }
 size_t pc_query_workspace(int nq) { return query_layout(nq).total; }
 size_t f64_reduce_workspace() { return al256(sizeof(SelState)) + al256(256 * 4) + al256(RED_BLOCKS * 8); }
 
+size_t radix_sort_hist_bytes(int n) { return static_cast<size_t>(sort_tiles(n)) * 256 * 4 + 4096 * 4; }
+
+cudaError_t launch_radix_sort(unsigned long long* keys[2], int* vals[2], int n, int bits, uint32_t* hist, int* in_b,
+                              cudaStream_t st) {
+  return radix_sort(keys, vals, n, bits, hist, in_b, st);
+}
+
 cudaError_t launch_pc_index_build(const void* pts, int f64, int n, void* index, cudaStream_t st) {
   const IndexLayout l = index_layout(n);
   uint8_t* b = static_cast<uint8_t*>(index);

@@ -119,6 +119,15 @@ _API = {
     "f3r_pnp_score": (C.c_int, [_P, _P, _P, _P, _I32, _P, _I32, _F32, _P, _P, _SIZE, _P]),
     "f3r_pnp_inliers_workspace": (_SIZE, [_I32, _I32]),
     "f3r_pnp_inliers": (C.c_int, [_P, _P, _P, _P, _I32, _P, _I32, _F32, _P, _P, _P, _P, _SIZE, _P]),
+    "f3r_sky_mask_workspace": (_SIZE, [_I32, _I32, _I32]),
+    "f3r_sky_mask": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _SIZE, _P]),
+    "f3r_scene_sort_workspace": (_SIZE, [_I32]),
+    "f3r_scene_sort": (C.c_int, [_P, _P, _P, _P, _P, _I32, _I32, _P, _P, _P, _P, _P, _SIZE, _P]),
+    "f3r_scene_visible_workspace": (_SIZE, [_I32, _SIZE]),
+    "f3r_scene_visible": (C.c_int, [_P, _I32, _SIZE, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _P, _SIZE, _P]),
+    "f3r_ply_pack": (C.c_int, [_P, _P, _SIZE, _P, _P]),
+    "f3r_extent_percentiles_workspace": (_SIZE, []),
+    "f3r_extent_percentiles": (C.c_int, [_P, _SIZE, _SIZE, _SIZE, _F32, _F32, _P, _P, _SIZE, _P]),
 }
 EXPORTS = list(_API)
 

@@ -476,6 +476,116 @@ def pnp_inliers(pts: torch.Tensor, pix: torch.Tensor, offsets, view_counts, hyps
     return out_pts[:m], out_pix[:m], counts
 
 
+# ------------------------------------------------------------------ viewer scene (csrc/scene.cu)
+I8, U8 = torch.int8, torch.uint8
+
+
+def sky_mask(img: torch.Tensor, out: Optional[torch.Tensor] = None):
+    """detect_sky_mask of each image of img fp32 [frames, 3, H, W] in [-1, 1].  Returns (not_sky int8 [frames, H W],
+    not-sky counts int32 [frames]); `out` (int8 [frames, H W]) receives the masks if given."""
+    _chk(img, F32, "img")
+    frames, three, h, w = img.shape
+    assert three == 3
+    if out is None:
+        out = torch.empty(frames, h * w, dtype=I8, device=img.device)
+    _chk(out, I8, "out")
+    assert out.shape == (frames, h * w)
+    counts = torch.empty(frames, dtype=torch.int32, device=img.device)
+    nbytes = L.load().f3r_sky_mask_workspace(frames, h, w)
+    ws = _scratch(nbytes, img.device)
+    # the reference's Python doubles: rows < int(H * 0.4) take the upper-rows rule; sky components need > H W 0.01 pixels
+    upper, min_sky = int(h * 0.4), int(np.floor(h * w * 0.01)) + 1
+    _call("f3r_sky_mask", img, _ptr(img), frames, h, w, upper, min_sky, _ptr(out), _ptr(counts), _ptr(ws), nbytes)
+    return out, counts
+
+
+def scene_sort(conf: torch.Tensor, pts: torch.Tensor, img: torch.Tensor, not_sky: torch.Tensor, offsets: torch.Tensor,
+               out_pts: torch.Tensor, out_rgb: torch.Tensor, out_not_sky: torch.Tensor, max_conf: torch.Tensor) -> None:
+    """One group of frames (frame f = elements offsets[f]:offsets[f + 1], offsets int64 on the device): each frame in
+    the order of np.argsort(-conf, kind="stable"), with its points fp32 [n, 3], u8 colours from the planar images img
+    (frame f's [3, hw] at 3 offsets[f]) and not-sky int8 [n] gathered into out_pts / out_rgb [n, 3] / out_not_sky [n];
+    max_conf fp32 [frames] gets each frame's conf.max()."""
+    n, frames = conf.numel(), offsets.numel() - 1
+    _chk(conf, F32, "conf"); _chk(pts, F32, "pts"); _chk(img, F32, "img"); _chk(not_sky, I8, "not_sky")
+    _chk(offsets, torch.int64, "offsets"); _chk(out_pts, F32, "out_pts"); _chk(out_rgb, U8, "out_rgb")
+    _chk(out_not_sky, I8, "out_not_sky"); _chk(max_conf, F32, "max_conf")
+    assert pts.numel() == 3 * n and img.numel() == 3 * n and not_sky.numel() == n and frames >= 1
+    assert out_pts.numel() == 3 * n and out_rgb.numel() == 3 * n and out_not_sky.numel() == n and max_conf.numel() == frames
+    nbytes = L.load().f3r_scene_sort_workspace(n)
+    ws = _scratch(nbytes, conf.device)
+    _call("f3r_scene_sort", conf, _ptr(conf), _ptr(pts), _ptr(img), _ptr(not_sky), _ptr(offsets), frames, n,
+          _ptr(out_pts), _ptr(out_rgb), _ptr(out_not_sky), _ptr(max_conf), _ptr(ws), nbytes)
+
+
+def scene_visible(segs: np.ndarray, pts_g: torch.Tensor, pts_l: torch.Tensor, rgb_g: torch.Tensor, rgb_l: torch.Tensor,
+                  not_sky_g: torch.Tensor, not_sky_l: torch.Tensor, mask_sky: bool):
+    """The rows of the segments segs (host int64 [nseg, 4]: head 0 global / 1 local, first row, row count, colour -1 for
+    the rows' own RGB or 0xRRGGBB) of the frame arrays, without the sky rows if mask_sky, segment after segment.
+    Returns (points fp32 [m, 3], colours uint8 [m, 3]) on the device."""
+    segs = np.ascontiguousarray(segs, dtype=np.int64).reshape(-1, 4)
+    dev = pts_g.device
+    if len(segs) == 0 or int(segs[:, 2].max()) == 0:
+        return torch.empty(0, 3, dtype=F32, device=dev), torch.empty(0, 3, dtype=U8, device=dev)
+    for t, dt, name in ((pts_g, F32, "pts_g"), (pts_l, F32, "pts_l"), (rgb_g, U8, "rgb_g"), (rgb_l, U8, "rgb_l"),
+                        (not_sky_g, I8, "not_sky_g"), (not_sky_l, I8, "not_sky_l")):
+        _chk(t, dt, name)
+    rows = (pts_g.shape[0], pts_l.shape[0])
+    if (segs[:, 1] < 0).any() or (segs[:, 2] < 0).any() or any(
+            int(s[1] + s[2]) > rows[int(s[0])] for s in segs) or not np.isin(segs[:, 0], (0, 1)).all():
+        raise ValueError("scene_visible: a segment reaches past its frame arrays")
+    nseg, max_len = len(segs), int(segs[:, 2].max())
+    nbytes = L.load().f3r_scene_visible_workspace(nseg, max_len)
+    ws = _scratch(nbytes, dev)
+    segs_d = torch.from_numpy(segs).to(dev)
+    total = torch.empty(1, dtype=torch.int64, device=dev)
+    args = (_ptr(pts_g), _ptr(pts_l), _ptr(rgb_g), _ptr(rgb_l), _ptr(not_sky_g), _ptr(not_sky_l), int(bool(mask_sky)))
+    _call("f3r_scene_visible", pts_g, _ptr(segs_d), nseg, max_len, *args, _ptr(total), None, None, _ptr(ws), nbytes)
+    m = int(total.item())
+    out_pts = torch.empty(m, 3, dtype=F32, device=dev)
+    out_rgb = torch.empty(m, 3, dtype=U8, device=dev)
+    if m:
+        _call("f3r_scene_visible", pts_g, _ptr(segs_d), nseg, max_len, *args, None, _ptr(out_pts), _ptr(out_rgb),
+              _ptr(ws), nbytes)
+    return out_pts, out_rgb
+
+
+def ply_pack(points: torch.Tensor, colors: torch.Tensor) -> torch.Tensor:
+    """uint8 [n * 15]: the little-endian PLY records (x, y, z float32, red, green, blue uint8) of the points."""
+    _chk(points, F32, "points"); _chk(colors, U8, "colors")
+    n = points.shape[0]
+    assert points.shape == (n, 3) and colors.shape == (n, 3)
+    out = torch.empty(15 * n, dtype=U8, device=points.device)
+    if n:
+        _call("f3r_ply_pack", points, _ptr(points), _ptr(colors), n, _ptr(out))
+    return out
+
+
+def percentile_plan(n: int, p: float):
+    """(lower rank, float32 weight) of np.percentile(x, p) for n float32 values, as numpy 2 forms them for method
+    "linear": q = p / float32(100) in float32, virtual index (n - 1) q in float32, the ranks floor and floor + 1 (both
+    n - 1 past the end), weight = virtual index - lower rank as numpy returns it from its index rule."""
+    q = np.true_divide(p, np.float32(100))
+    v = np.float32(n - 1) * q
+    prev = int(np.floor(v))
+    if v >= n - 1:
+        return n - 1, np.float32(v - np.float32(-1))  # numpy marks both ranks -1 there; the weight meets equal bounds
+    return prev, np.float32(v - np.float32(prev))
+
+
+def extent_percentiles(points: torch.Tensor, lo: float = 20, hi: float = 80) -> torch.Tensor:
+    """fp32 [7] on the device: np.percentile(points, lo, axis=0), np.percentile(points, hi, axis=0) and the largest
+    per-axis difference hi - lo (NaN for an axis holding a NaN), for points fp32 [n, 3], n >= 1."""
+    _chk(points, F32, "points")
+    n = points.shape[0]
+    assert points.shape == (n, 3) and n >= 1
+    (k0, g0), (k1, g1) = percentile_plan(n, lo), percentile_plan(n, hi)
+    nbytes = L.load().f3r_extent_percentiles_workspace()
+    ws = _scratch(nbytes, points.device)
+    out = torch.empty(7, dtype=F32, device=points.device)
+    _call("f3r_extent_percentiles", points, _ptr(points), n, k0, k1, float(g0), float(g1), _ptr(out), _ptr(ws), nbytes)
+    return out
+
+
 # ------------------------------------------------------------------ reconstruction metrics (csrc/pointcloud.cu)
 F64 = torch.float64
 

@@ -311,6 +311,49 @@ int f3r_pnp_inliers(const float* pts, const float* pix, const int64_t* offsets, 
                     const f3r_pnp_hyp* hyps, int32_t nh, float thr, float* out_pts, float* out_pix, int32_t* out_counts,
                     void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- viewer scene: the frame preparation and the point export of the reference's viewer
+ * (fast3r/viz/viser_visualizer.py:24-72, :168-254, :343-427), exact with respect to numpy / cv2 / scipy.  The host
+ * groups the frames, applies the viewer's settings and writes the PLY header (fast3r_b200/scene.py).
+ *
+ * f3r_sky_mask: detect_sky_mask of `frames` images of one shape, img [frames][3][h][w] (fp32 in [-1, 1]): u8
+ *   ((x + 1) * 127.5, truncated), OpenCV's 8-bit RGB -> HSV, the three inRange boxes, S < 50 and V > 150 in rows
+ *   < upper_rows (= int(h * 0.4)), a 7x7 dilate then a 7x7 open, 4-connected components; sky = the components touching
+ *   row 0 of >= min_sky (= floor(h w 0.01) + 1) pixels, or the whole mask if none touches row 0.  not_sky [frames][h][w]
+ *   (int8 0/1) and not_sky_count [frames] (int32).  workspace: f3r_sky_mask_workspace(frames, h, w) bytes, 256-byte
+ *   aligned.
+ * f3r_scene_sort: one group of frames, frame f = elements [offsets[f], offsets[f + 1]) (offsets: DEVICE int64
+ *   [frames + 1], offsets[0] = 0, offsets[frames] = n): each frame in the order of np.argsort(-conf, kind="stable")
+ *   (descending, -0.0 == +0.0, NaN last, ties by index).  Slot j of that order gets the point (pts [n][3]), the u8
+ *   colour of the pixel (img: frame f's planar [3][hw] image at 3 offsets[f]) and its not-sky value into out_pts
+ *   [n][3], out_rgb [n][3], out_not_sky [n]; max_conf [frames] gets conf.max() of each frame (NaN if it holds a NaN).
+ *   workspace: f3r_scene_sort_workspace(n) bytes, 256-byte aligned.
+ * f3r_scene_visible: segments segs [nseg][4] (DEVICE int64: head 0 = global / 1 = local, first row, row count <=
+ *   max_len, colour -1 = the rows' own RGB or 0xRRGGBB) of the frame arrays pts_* [.][3], rgb_* [.][3], not_sky_*;
+ *   with mask_sky only rows of not_sky > 0.  Two calls on one workspace: with total (DEVICE uint64) the count of kept
+ *   rows; then with out_pts [total][3] and out_rgb [total][3] the kept rows, segment after segment in row order.
+ *   workspace: f3r_scene_visible_workspace(nseg, max_len) bytes, 256-byte aligned.
+ * f3r_ply_pack: out [n][15] = the binary_little_endian PLY records of the points (3 x float32, 3 x uint8).
+ * f3r_extent_percentiles: out[7] = np.percentile(pts, 20 and 80, axis=0) for pts [n][3] (float32, method "linear") as
+ *   out[0..2] and out[3..5], and out[6] = max over axes of out[3 + a] - out[a].  The host gives each percentile's lower
+ *   rank k0 / k1 and float32 weight g0 / g1 as numpy forms them; a column holding a NaN gives NaN.  workspace:
+ *   f3r_extent_percentiles_workspace() bytes, 256-byte aligned. */
+size_t f3r_sky_mask_workspace(int32_t frames, int32_t h, int32_t w);
+int f3r_sky_mask(const float* img, int32_t frames, int32_t h, int32_t w, int32_t upper_rows, int32_t min_sky,
+                 int8_t* not_sky, int32_t* not_sky_count, void* workspace, size_t workspace_bytes, void* stream);
+size_t f3r_scene_sort_workspace(int32_t n);
+int f3r_scene_sort(const float* conf, const float* pts, const float* img, const int8_t* not_sky, const int64_t* offsets,
+                   int32_t frames, int32_t n, float* out_pts, uint8_t* out_rgb, int8_t* out_not_sky, float* max_conf,
+                   void* workspace, size_t workspace_bytes, void* stream);
+size_t f3r_scene_visible_workspace(int32_t nseg, size_t max_len);
+int f3r_scene_visible(const int64_t* segs, int32_t nseg, size_t max_len, const float* pts_g, const float* pts_l,
+                      const uint8_t* rgb_g, const uint8_t* rgb_l, const int8_t* not_sky_g, const int8_t* not_sky_l,
+                      int32_t mask_sky, uint64_t* total, float* out_pts, uint8_t* out_rgb, void* workspace,
+                      size_t workspace_bytes, void* stream);
+int f3r_ply_pack(const float* pts, const uint8_t* rgb, size_t n, uint8_t* out, void* stream);
+size_t f3r_extent_percentiles_workspace(void);
+int f3r_extent_percentiles(const float* pts, size_t n, size_t k0, size_t k1, float g0, float g1, float* out,
+                           void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
