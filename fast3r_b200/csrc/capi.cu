@@ -675,6 +675,42 @@ int f3r_pnp_inliers(const float* pts, const float* pix, const int64_t* offsets, 
                "f3r_pnp_inliers");
 }
 
+// ---------------------------------------------------------------- camera-pose metric
+static bool pose_metric_shape_ok(int32_t items, int32_t views) {
+  return items >= 1 && items <= 65535 && views >= 2 && views <= 65536 &&
+         static_cast<long long>(items) * views < (1ll << 31);
+}
+
+size_t f3r_pose_metric_workspace(int32_t f64, int32_t items, int32_t views) {
+  return pose_metric_shape_ok(items, views) ? f3r::pose_metric_workspace(f64 != 0, items, views) : 0;
+}
+
+int f3r_pose_metric(int32_t f64, const void* pred, const void* gt, int32_t items, int32_t views, int32_t hist_max,
+                    void* r_out, void* t_out, int64_t* counts, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!pred || !gt || !counts || !workspace) return fail("f3r_pose_metric: null operand");
+  if ((r_out != nullptr) != (t_out != nullptr)) return fail("f3r_pose_metric: give both of r_out and t_out or neither");
+  if (!pose_metric_shape_ok(items, views)) return fail("f3r_pose_metric: bad shape items=%d views=%d", items, views);
+  if (hist_max < 1 || hist_max >= F3R_PM_MAX_BINS) return fail("f3r_pose_metric: hist_max %d not in [1, %d)", hist_max,
+                                                               F3R_PM_MAX_BINS);
+  if (workspace_bytes < f3r::pose_metric_workspace(f64 != 0, items, views))
+    return fail("f3r_pose_metric: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 7) return fail("f3r_pose_metric: workspace not 8-byte aligned");
+  return check(f3r::launch_pose_metric(f64 != 0, pred, gt, items, views, hist_max, r_out, t_out,
+                                       reinterpret_cast<unsigned long long*>(counts), workspace,
+                                       static_cast<cudaStream_t>(stream)), "f3r_pose_metric");
+}
+
+int f3r_pose_metric_counts(int32_t f64, const void* r, const void* t, size_t n, int32_t hist_max, int64_t* counts,
+                           void* stream) {
+  if (!counts || (n && (!r || !t))) return fail("f3r_pose_metric_counts: null operand");
+  if (n > (1ull << 40)) return fail("f3r_pose_metric_counts: %zu angles (at most 2^40)", n);
+  if (hist_max < 1 || hist_max >= F3R_PM_MAX_BINS) return fail("f3r_pose_metric_counts: hist_max %d not in [1, %d)",
+                                                               hist_max, F3R_PM_MAX_BINS);
+  return check(f3r::launch_pose_metric_counts(f64 != 0, r, t, static_cast<long long>(n), hist_max,
+                                              reinterpret_cast<unsigned long long*>(counts),
+                                              static_cast<cudaStream_t>(stream)), "f3r_pose_metric_counts");
+}
+
 // ---------------------------------------------------------------- viewer scene
 static bool sky_shape_ok(int32_t frames, int32_t h, int32_t w) {
   return frames > 0 && h > 0 && w > 0 && static_cast<long long>(frames) * h * w < (1ll << 31);

@@ -203,6 +203,15 @@ cudaError_t launch_pnp_inliers(const float* pts, const float* pix, const long lo
                                const f3r_pnp_hyp* hyps, int nh, float thr, float* out_pts, float* out_pix, int* counts,
                                void* workspace, cudaStream_t stream);
 
+// camera-pose metric (pose_metric.cu); counts: [items][PM_COUNTS] (F3R_PM_* of include/fast3r_b200.h)
+constexpr int PM_FLAGS = F3R_PM_HIST;
+constexpr int PM_MAX_BINS = F3R_PM_MAX_BINS;
+constexpr int PM_COUNTS = F3R_PM_COUNTS;
+size_t pose_metric_workspace(int f64, int items, int views);
+cudaError_t launch_pose_metric(int f64, const void* pred, const void* gt, int items, int views, int hmax, void* r_out,
+                               void* t_out, unsigned long long* counts, void* workspace, cudaStream_t stream);
+cudaError_t launch_pose_metric_counts(int f64, const void* r, const void* t, long long n, int hmax,
+                                      unsigned long long* counts, cudaStream_t stream);
 
 // viewer scene (scene.cu)
 size_t sky_mask_workspace(int frames, int h, int w);

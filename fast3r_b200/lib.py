@@ -52,6 +52,12 @@ PNP_HYP = np.dtype([("r", "<f8", (9,)), ("t", "<f8", (3,)), ("fx", "<f8"), ("fy"
                     ("view", "<i4"), ("reserved", "<i4")])
 
 
+# f3r_pose_metric's counts row: [0..2] rotation angle < 5 / 15 / 30, [3..5] translation angle < 5 / 15 / 30, [6] bad
+# traces, [7] pairs, [PM_HIST + b] histogram bin b
+PM_HIST, PM_MAX_BINS = 8, 64
+PM_COUNTS = PM_HIST + PM_MAX_BINS
+
+
 class JpegInfo(C.Structure):
     _fields_ = [("status", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("components", C.c_int32),
                 ("h_samp", C.c_int32), ("v_samp", C.c_int32), ("restart_interval", C.c_int32), ("segments", C.c_int32),
@@ -119,6 +125,9 @@ _API = {
     "f3r_pnp_score": (C.c_int, [_P, _P, _P, _P, _I32, _P, _I32, _F32, _P, _P, _SIZE, _P]),
     "f3r_pnp_inliers_workspace": (_SIZE, [_I32, _I32]),
     "f3r_pnp_inliers": (C.c_int, [_P, _P, _P, _P, _I32, _P, _I32, _F32, _P, _P, _P, _P, _SIZE, _P]),
+    "f3r_pose_metric_workspace": (_SIZE, [_I32, _I32, _I32]),
+    "f3r_pose_metric": (C.c_int, [_I32, _P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _SIZE, _P]),
+    "f3r_pose_metric_counts": (C.c_int, [_I32, _P, _P, _SIZE, _I32, _P, _P]),
     "f3r_sky_mask_workspace": (_SIZE, [_I32, _I32, _I32]),
     "f3r_sky_mask": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _SIZE, _P]),
     "f3r_scene_sort_workspace": (_SIZE, [_I32]),

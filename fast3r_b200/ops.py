@@ -476,6 +476,41 @@ def pnp_inliers(pts: torch.Tensor, pix: torch.Tensor, offsets, view_counts, hyps
     return out_pts[:m], out_pix[:m], counts
 
 
+# ------------------------------------------------------------------ camera-pose metric (csrc/pose_metric.cu)
+def pose_metric(pred: torch.Tensor, gt: torch.Tensor, hist_max: int = 30, angles: bool = False):
+    """pred, gt [items, views, 4, 4] cam-to-world, both float32 or both float64.  Returns (counts int64 [items,
+    lib.PM_COUNTS], r, t): the counts row of f3r_pose_metric per item and, with `angles`, the rotation and translation
+    angles in degrees [items, views (views - 1) / 2] of every pair in torch.combinations order (else None, None)."""
+    if pred.dtype not in (F32, torch.float64) or gt.dtype != pred.dtype:
+        raise TypeError(f"pose_metric: pred and gt must both be float32 or both float64, got {pred.dtype} and {gt.dtype}")
+    _chk(pred, pred.dtype, "pred"); _chk(gt, pred.dtype, "gt")
+    items, views = pred.shape[0], pred.shape[1]
+    assert pred.shape == (items, views, 4, 4) and gt.shape == pred.shape
+    f64 = int(pred.dtype == torch.float64)
+    nbytes = L.load().f3r_pose_metric_workspace(f64, items, views)
+    ws = _scratch(nbytes, pred.device)
+    counts = torch.empty(items, L.PM_COUNTS, dtype=torch.int64, device=pred.device)
+    r = t = None
+    if angles:
+        r = torch.empty(items, views * (views - 1) // 2, dtype=pred.dtype, device=pred.device)
+        t = torch.empty_like(r)
+    _call("f3r_pose_metric", pred, f64, _ptr(pred), _ptr(gt), items, views, int(hist_max), _ptr(r), _ptr(t),
+          _ptr(counts), _ptr(ws), nbytes)
+    return counts, r, t
+
+
+def pose_metric_counts(r: torch.Tensor, t: torch.Tensor, hist_max: int = 30) -> torch.Tensor:
+    """The counts row (int64 [lib.PM_COUNTS]) of given angle vectors r, t [n] (both float32 or both float64)."""
+    if r.dtype not in (F32, torch.float64) or t.dtype != r.dtype:
+        raise TypeError(f"pose_metric_counts: r and t must both be float32 or both float64, got {r.dtype} and {t.dtype}")
+    _chk(r, r.dtype, "r"); _chk(t, r.dtype, "t")
+    assert r.dim() == 1 and t.shape == r.shape
+    counts = torch.empty(L.PM_COUNTS, dtype=torch.int64, device=r.device)
+    _call("f3r_pose_metric_counts", r, int(r.dtype == torch.float64), _ptr(r), _ptr(t), r.numel(), int(hist_max),
+          _ptr(counts))
+    return counts
+
+
 # ------------------------------------------------------------------ viewer scene (csrc/scene.cu)
 I8, U8 = torch.int8, torch.uint8
 

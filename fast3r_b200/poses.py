@@ -348,7 +348,8 @@ def estimate_camera_poses(preds, views=None, niter_PnP=10, focal_length_estimati
         focal = None
         if focal_length_estimation_method in keys:
             kp, kc = keys[focal_length_estimation_method]
-            focal = estimate_focal(preds[0][kp][i:i + 1], preds[0][kc][i:i + 1], min_conf_thr_percentile=10)
+            # [i][None], not [i:i + 1]: correct_preds_orientation leaves lists of per-item tensors
+            focal = estimate_focal(preds[0][kp][i][None], preds[0][kc][i][None], min_conf_thr_percentile=10)
         items += [(p["pts3d_in_other_view"][i], p["conf"][i], focal) for p in preds]
     with _pool() as pool:
         res = _run_views(items, niter_PnP, pool)

@@ -15,6 +15,9 @@ Same names, arguments and results as the reference:
 
 * ``fast_pnp``, ``estimate_cam_pose_one_sample`` and ``estimate_camera_poses`` - the camera poses, re-exported from
   fast3r_b200.poses (RANSAC scoring on the GPU, bit-identical to cv2.solvePnPRansac).
+* ``correct_preds_orientation(preds, views)`` and ``evaluate_camera_poses(views, preds, niter_PnP=10,
+  focal_length_estimation_method='individual')`` - multiview_dust3r_module.py:871-937 and :737-804: RRA / RTA / mAA
+  per batch item, all pairs of all items in one launch (fast3r_b200.cam_pose_metric).
 
 NOT here (documented in DESIGN.md §1): the "median" focal mode.  Tensors may live on the CPU (what ``inference()`` returns) or on a CUDA device; CPU inputs are
 copied to ``device`` (default cuda:0) and the results copied back, so the function is a drop-in either way.  There is
@@ -172,3 +175,56 @@ def _registered_clouds(views, preds, i: int, pct_icp: float, pct_metric: float, 
     rts = ops.similarity_fit(xs, ys, None, None, weights.reshape(1, nv * n).to(torch.uint8).contiguous())
     aligned = ops.similarity_apply(xs, rts)[0]
     return aligned[mask_pred.reshape(-1)].contiguous(), y[valid].contiguous(), rts[0]
+
+
+def correct_preds_orientation(preds: List[Dict], views: List[Dict]) -> None:
+    """MultiViewDUSt3RLitModule.correct_preds_orientation (multiview_dust3r_module.py:871-937), in place: the items whose
+    true_shape (H, W) is portrait get their pointmaps and confidences transposed back (the data loader transposed
+    them to landscape), and those entries become lists of per-item tensors."""
+    if views is None:
+        return
+    for pred, view in zip(preds, views):
+        portrait = [bool(h > w) for h, w in view["true_shape"].tolist()]
+        keys = ["conf", "pts3d_in_other_view"]
+        if "pts3d_local" in pred:
+            keys += ["conf_local", "pts3d_local"] + (["pts3d_local_aligned_to_global"]
+                                                     if "pts3d_local_aligned_to_global" in pred else [])
+        for key in keys:
+            pred[key] = [x.transpose(0, 1) if p else x for x, p in zip(pred[key], portrait)]
+
+
+def evaluate_camera_poses(views: List[Dict], preds: List[Dict], niter_PnP: int = 10,
+                          focal_length_estimation_method: str = "individual", device=None) -> List[Dict]:
+    """MultiViewDUSt3RLitModule.evaluate_camera_poses (multiview_dust3r_module.py:737-804) without the Lightning side:
+    returns one dict of RRA_at_{5,15,30}, RTA_at_{5,15,30} and mAA_30 (python floats) per batch item instead of
+    logging them.
+
+    The first-view-from-local-head alignment, the in-place portrait correction and estimate_camera_poses run as in the
+    reference; the estimated poses are cast to the dtype of the ground-truth camera_pose and every pair of every item
+    is scored in one launch (fast3r_b200.cam_pose_metric).  Two differences: with fewer than 2 views this raises
+    ValueError (the reference logs a warning and then fails on an unbound name), and nothing is printed per item."""
+    import numpy as np
+
+    from . import cam_pose_metric as cpm
+    from . import lib as L
+    if focal_length_estimation_method == "first_view_from_local_head":
+        align_local_pts3d_to_global(preds, views, device=device)
+    correct_preds_orientation(preds, views)
+    poses_c2w, _ = estimate_camera_poses(preds=preds, views=views, niter_PnP=niter_PnP,
+                                         focal_length_estimation_method=focal_length_estimation_method)
+    gt_list = [view["camera_pose"] for view in views]
+    pred_cameras = torch.tensor(np.stack(poses_c2w), dtype=gt_list[0].dtype)   # (B, N, 4, 4)
+    gt_cameras = torch.stack(gt_list).transpose(0, 1)                           # (B, N, 4, 4)
+    nv = pred_cameras.shape[1]
+    if nv < 2:
+        raise ValueError("Not enough camera poses to compute relative errors.")
+    counts, _, _ = cpm.pose_counts(pred_cameras, gt_cameras, device)
+    pairs = nv * (nv - 1) // 2
+    results = []
+    for row in counts.tolist():
+        res = {f"RRA_at_{tau}": cpm.below_ratio(row[k], pairs) for k, tau in enumerate(cpm.RRA_THRESHOLDS)}
+        res.update({f"RTA_at_{tau}": cpm.below_ratio(row[3 + k], pairs) for k, tau in enumerate(cpm.RTA_THRESHOLDS)})
+        hist = torch.tensor(row[L.PM_HIST:L.PM_HIST + 31], dtype=gt_cameras.dtype)
+        res["mAA_30"] = cpm.auc_from_hist(hist, pairs).item()
+        results.append(res)
+    return results

@@ -311,6 +311,28 @@ int f3r_pnp_inliers(const float* pts, const float* pix, const int64_t* offsets, 
                     const f3r_pnp_hyp* hyps, int32_t nh, float thr, float* out_pts, float* out_pix, int32_t* out_counts,
                     void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- camera-pose metric: the relative-pose errors of all view pairs behind evaluate_camera_poses' RRA / RTA / mAA
+ * (fast3r/eval/cam_pose_metric.py camera_to_rel_deg / calculate_auc with fast3r/utils/so3_utils.py), in the
+ * reference's CPU arithmetic (fast3r_b200/csrc/pose_metric_math.h); the host forms the means (fast3r_b200/cam_pose_metric.py).
+ *
+ * f3r_pose_metric: pred and gt [items][views][4][4] (row-major cam-to-world, float32 or float64 by f64; DEVICE), pairs
+ *   (i, j), i < j, in torch.combinations order, P = views (views - 1) / 2 per item.  Per pair: the rotation angle of
+ *   R_gt R_pred^T and the translation angle of the relative poses inv(pose_i) pose_j, in degrees.  r_out / t_out
+ *   [items][P] (same type; both NULL or both given) receive them.  counts [items][F3R_PM_COUNTS] (int64) receive: [0..2]
+ *   pairs with rotation angle < 5, 15, 30; [3..5] translation angle < 5, 15, 30; [6] pairs whose trace is outside
+ *   [-1 - 1e-4, 3 + 1e-4] (NaN is not); [7] pairs counted (= P); [F3R_PM_HIST + b] torch.histc(max(r, t),
+ *   bins = hist_max + 1, min = 0, max = hist_max) bin b.  1 <= hist_max < F3R_PM_MAX_BINS; 2 <= views <= 65536;
+ *   1 <= items <= 65535, items * views < 2^31.  workspace: f3r_pose_metric_workspace(f64, items, views) bytes, 8-byte aligned.
+ * f3r_pose_metric_counts: the counts of one item ([6] = 0) from given angles r, t [n] (DEVICE). */
+#define F3R_PM_HIST 8
+#define F3R_PM_MAX_BINS 64
+#define F3R_PM_COUNTS (F3R_PM_HIST + F3R_PM_MAX_BINS)
+size_t f3r_pose_metric_workspace(int32_t f64, int32_t items, int32_t views);
+int f3r_pose_metric(int32_t f64, const void* pred, const void* gt, int32_t items, int32_t views, int32_t hist_max,
+                    void* r_out, void* t_out, int64_t* counts, void* workspace, size_t workspace_bytes, void* stream);
+int f3r_pose_metric_counts(int32_t f64, const void* r, const void* t, size_t n, int32_t hist_max, int64_t* counts,
+                           void* stream);
+
 /* ---- viewer scene: the frame preparation and the point export of the reference's viewer
  * (fast3r/viz/viser_visualizer.py:24-72, :168-254, :343-427), exact with respect to numpy / cv2 / scipy.  The host
  * groups the frames, applies the viewer's settings and writes the PLY header (fast3r_b200/scene.py).
