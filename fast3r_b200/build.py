@@ -7,8 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfast3r_b200.so")
 SOURCES = ["capi.cu", "gemm.cu", "attention.cu", "attention_x3.cu", "elementwise.cu", "ingest.cu", "geometry.cu", "jpeg.cu",
-           "pointcloud.cu", "pose.cu", "pose_metric.cu", "scene.cu"]
-HEADERS = ["common.cuh", "f3r_kernels.h", "gemm_plan.h", "geometry_math.h", "jpeg_math.h", "jpeg_parse.h", "pointcloud_math.h", "pose_math.h", "pose_metric_math.h", "scene_math.h",
+           "pointcloud.cu", "pose.cu", "pose_metric.cu", "scene.cu", "val_loss.cu"]
+HEADERS = ["common.cuh", "f3r_kernels.h", "gemm_plan.h", "geometry_math.h", "jpeg_math.h", "jpeg_parse.h", "pointcloud_math.h", "pose_math.h", "pose_metric_math.h", "scene_math.h", "val_loss_math.h",
            os.path.join("..", "..", "include", "fast3r_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC"]

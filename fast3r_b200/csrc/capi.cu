@@ -1,6 +1,7 @@
 // extern "C" boundary of libfast3r_b200.so (see include/fast3r_b200.h).  Builds the TMA descriptors
 // (cuTensorMapEncodeTiled through cudaGetDriverEntryPoint, so libcuda is not a link-time dependency),
 // validates arguments and enqueues the kernels on the caller's stream.
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -709,6 +710,31 @@ int f3r_pose_metric_counts(int32_t f64, const void* r, const void* t, size_t n, 
   return check(f3r::launch_pose_metric_counts(f64 != 0, r, t, static_cast<long long>(n), hist_max,
                                               reinterpret_cast<unsigned long long*>(counts),
                                               static_cast<cudaStream_t>(stream)), "f3r_pose_metric_counts");
+}
+
+// ---------------------------------------------------------------- validation criterion
+static bool val_loss_shape_ok(int32_t views, int32_t items, int32_t n) {
+  return views >= 1 && items >= 1 && n >= 1 && static_cast<long long>(views) * items * n < (1ll << 31);
+}
+
+size_t f3r_val_loss_workspace(int32_t views, int32_t items, int32_t n) {
+  return val_loss_shape_ok(views, items, n) ? f3r::val_loss_workspace(views, items, n) : 0;
+}
+
+int f3r_val_loss(const float* gt, const uint8_t* valid, const float* pr, const float* pr_local, const float* conf,
+                 const float* conf_local, const float* poses, int32_t views, int32_t items, int32_t n, float alpha,
+                 int32_t log1p, int32_t gt_scale, int32_t local_scale_consistent, int32_t has_local, double* out,
+                 void* workspace, size_t workspace_bytes, void* stream) {
+  if (!gt || !valid || !pr || !conf || !poses || !out || !workspace) return fail("f3r_val_loss: null operand");
+  if (has_local && (!pr_local || !conf_local)) return fail("f3r_val_loss: has_local needs pr_local and conf_local");
+  if (!val_loss_shape_ok(views, items, n))
+    return fail("f3r_val_loss: bad shape views=%d items=%d n=%d (views * items * n must be below 2^31)", views, items, n);
+  if (!(alpha > 0.f) || !std::isfinite(alpha)) return fail("f3r_val_loss: alpha must be positive and finite");
+  if (workspace_bytes < f3r::val_loss_workspace(views, items, n)) return fail("f3r_val_loss: workspace too small");
+  if (reinterpret_cast<uintptr_t>(workspace) & 7) return fail("f3r_val_loss: workspace not 8-byte aligned");
+  return check(f3r::launch_val_loss(gt, valid, pr, pr_local, conf, conf_local, poses, views, items, n, alpha, log1p != 0,
+                                    gt_scale != 0, local_scale_consistent != 0, has_local != 0, out, workspace,
+                                    static_cast<cudaStream_t>(stream)), "f3r_val_loss");
 }
 
 // ---------------------------------------------------------------- viewer scene

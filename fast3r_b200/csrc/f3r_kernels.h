@@ -213,6 +213,13 @@ cudaError_t launch_pose_metric(int f64, const void* pred, const void* gt, int it
 cudaError_t launch_pose_metric_counts(int f64, const void* r, const void* t, long long n, int hmax,
                                       unsigned long long* counts, cudaStream_t stream);
 
+// validation criterion (val_loss.cu); out: [views][items][5] (val_loss_math.h vl::TERM_SUMS)
+size_t val_loss_workspace(int views, int items, int n);
+cudaError_t launch_val_loss(const float* gt, const uint8_t* valid, const float* pr, const float* pr_local,
+                            const float* conf, const float* conf_local, const float* poses, int views, int items,
+                            int n, float alpha, bool log1p, bool gt_scale, bool local_scale_consistent, bool has_local,
+                            double* out, void* workspace, cudaStream_t stream);
+
 // viewer scene (scene.cu)
 size_t sky_mask_workspace(int frames, int h, int w);
 cudaError_t launch_sky_mask(const float* img, int frames, int h, int w, int upper, int min_sky, int8_t* not_sky,

@@ -128,6 +128,9 @@ _API = {
     "f3r_pose_metric_workspace": (_SIZE, [_I32, _I32, _I32]),
     "f3r_pose_metric": (C.c_int, [_I32, _P, _P, _I32, _I32, _I32, _P, _P, _P, _P, _SIZE, _P]),
     "f3r_pose_metric_counts": (C.c_int, [_I32, _P, _P, _SIZE, _I32, _P, _P]),
+    "f3r_val_loss_workspace": (_SIZE, [_I32, _I32, _I32]),
+    "f3r_val_loss": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _I32, _I32, _I32, _F32, _I32, _I32, _I32, _I32, _P, _P, _SIZE,
+                               _P]),
     "f3r_sky_mask_workspace": (_SIZE, [_I32, _I32, _I32]),
     "f3r_sky_mask": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I32, _P, _P, _P, _SIZE, _P]),
     "f3r_scene_sort_workspace": (_SIZE, [_I32]),

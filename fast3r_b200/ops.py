@@ -511,6 +511,39 @@ def pose_metric_counts(r: torch.Tensor, t: torch.Tensor, hist_max: int = 30) -> 
     return counts
 
 
+# ------------------------------------------------------------------ validation criterion (csrc/val_loss.cu)
+VL_SUMS = 5  # per (view, item): sum d and sum d c - alpha log c of the global term, the same of the local term, count
+
+
+def val_loss(gt: torch.Tensor, valid: torch.Tensor, pr: torch.Tensor, conf: torch.Tensor, poses: torch.Tensor,
+             pr_local: Optional[torch.Tensor] = None, conf_local: Optional[torch.Tensor] = None, alpha: float = 1.0,
+             log1p: bool = False, gt_scale: bool = False, local_scale_consistent: bool = False) -> torch.Tensor:
+    """The sums of f3r_val_loss (float64 [views, items, VL_SUMS], on the device) from maps stacked [views, items, n]:
+    gt, pr, pr_local float32 [..., 3], valid uint8, conf, conf_local float32, poses float32 [views, items, 4, 4].  The
+    local term runs when pr_local and conf_local are given."""
+    views, items, n = valid.shape
+    for t, name in ((gt, "gt"), (pr, "pr"), (pr_local, "pr_local")):
+        if t is not None:
+            _chk(t, F32, name)
+            assert t.shape == (views, items, n, 3), (name, t.shape)
+    for t, name in ((conf, "conf"), (conf_local, "conf_local")):
+        if t is not None:
+            _chk(t, F32, name)
+            assert t.shape == (views, items, n), (name, t.shape)
+    _chk(valid, torch.uint8, "valid"); _chk(poses, F32, "poses")
+    assert poses.shape == (views, items, 4, 4)
+    has_local = pr_local is not None
+    if has_local != (conf_local is not None):
+        raise ValueError("val_loss: give both of pr_local and conf_local or neither")
+    nbytes = L.load().f3r_val_loss_workspace(views, items, n)
+    ws = _scratch(nbytes, gt.device)
+    out = torch.empty(views, items, VL_SUMS, dtype=torch.float64, device=gt.device)
+    _call("f3r_val_loss", gt, _ptr(gt), _ptr(valid), _ptr(pr), _ptr(pr_local), _ptr(conf), _ptr(conf_local),
+          _ptr(poses), views, items, n, float(alpha), int(log1p), int(gt_scale), int(local_scale_consistent),
+          int(has_local), _ptr(out), _ptr(ws), nbytes)
+    return out
+
+
 # ------------------------------------------------------------------ viewer scene (csrc/scene.cu)
 I8, U8 = torch.int8, torch.uint8
 

@@ -333,6 +333,27 @@ int f3r_pose_metric(int32_t f64, const void* pred, const void* gt, int32_t items
 int f3r_pose_metric_counts(int32_t f64, const void* r, const void* t, size_t n, int32_t hist_max, int64_t* counts,
                            void* stream);
 
+/* ---- validation criterion: ConfLossMultiviewV2(Regr3DMultiviewV4(L21Loss())) of fast3r/dust3r/losses.py:570-848,
+ * forward only (fast3r_b200/csrc/val_loss.cu); the host forms the means, the loss and the details
+ * (fast3r_b200/losses.py).
+ *
+ * f3r_val_loss: every map is stacked [views][items][n] (DEVICE): gt [.][3] (pts3d), valid (uint8 0/1), pr [.][3]
+ *   (pts3d_in_other_view), conf, and with has_local pr_local [.][3] (pts3d_local) and conf_local (else NULL); poses
+ *   [views][items][4][4] (camera_pose, float32, row-major).  Ground truth goes to view 0's frame (global term) and to its
+ *   own view's frame (local term) through inverses formed in double.  Norm factors: the mean of ||p|| (log1p ||p|| with
+ *   log1p) over the valid pixels where it is not NaN, clipped below at 1e-8 - per item over all views for the global
+ *   term, per (view, item) for the local term, or the global ones with local_scale_consistent; with gt_scale the ground
+ *   truth keeps its scale.  out [views][items][5] (float64, DEVICE) receives per (view, item), over the valid pixels:
+ *   [0] sum of d = ||pr / f_pr - gt / f_gt|| and [1] sum of d c - alpha log c of the global term, [2] and [3] the same
+ *   of the local term (0 without has_local), [4] the number of valid pixels.  alpha > 0; views, items, n >= 1 and
+ *   views * items * n < 2^31.  workspace: f3r_val_loss_workspace(views, items, n) bytes, 8-byte aligned.  Two calls
+ *   on the same inputs give the same bits. */
+size_t f3r_val_loss_workspace(int32_t views, int32_t items, int32_t n);
+int f3r_val_loss(const float* gt, const uint8_t* valid, const float* pr, const float* pr_local, const float* conf,
+                 const float* conf_local, const float* poses, int32_t views, int32_t items, int32_t n, float alpha,
+                 int32_t log1p, int32_t gt_scale, int32_t local_scale_consistent, int32_t has_local, double* out,
+                 void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- viewer scene: the frame preparation and the point export of the reference's viewer
  * (fast3r/viz/viser_visualizer.py:24-72, :168-254, :343-427), exact with respect to numpy / cv2 / scipy.  The host
  * groups the frames, applies the viewer's settings and writes the PLY header (fast3r_b200/scene.py).
