@@ -817,6 +817,36 @@ int f3r_extent_percentiles(const float* pts, size_t n, size_t k0, size_t k1, flo
                                               static_cast<cudaStream_t>(stream)), "f3r_extent_percentiles");
 }
 
+// ---------------------------------------------------------------- ground-truth views
+int f3r_view_geometry(const f3r_view_param* params, const f3r_view_param* params_dev, int32_t count, float* out_pts,
+                      uint8_t* out_valid, float* out_depth, size_t out_pixels, void* stream) {
+  if (!params || !params_dev || !out_pts || !out_valid || !out_depth) return fail("f3r_view_geometry: null operand");
+  if (count < 1 || count > 65535) return fail("f3r_view_geometry: %d views (1 to 65535)", count);
+  if (out_pixels >= (1ull << 31)) return fail("f3r_view_geometry: %zu output pixels (below 2^31)", out_pixels);
+  int max_pixels = 0;
+  for (int i = 0; i < count; ++i) {
+    const f3r_view_param& p = params[i];
+    if (!p.depth) return fail("f3r_view_geometry: view %d: null depth", i);
+    if (reinterpret_cast<uintptr_t>(p.depth) & 3) return fail("f3r_view_geometry: view %d: depth not 4-byte aligned", i);
+    if (p.src_w <= 0 || p.src_h <= 0 || static_cast<long long>(p.src_w) * p.src_h >= (1ll << 31))
+      return fail("f3r_view_geometry: view %d: bad source size %dx%d", i, p.src_w, p.src_h);
+    if (p.crop_x < 0 || p.crop_y < 0 || p.crop_w <= 0 || p.crop_h <= 0 || p.crop_w > p.src_w - p.crop_x ||
+        p.crop_h > p.src_h - p.crop_y)
+      return fail("f3r_view_geometry: view %d: crop outside the source", i);
+    if (p.rs_w <= 0 || p.rs_h <= 0 || p.out_w <= 0 || p.out_h <= 0)
+      return fail("f3r_view_geometry: view %d: bad resized or output size", i);
+    if (p.box_x < 0 || p.box_y < 0 || p.out_w > p.rs_w - p.box_x || p.out_h > p.rs_h - p.box_y)
+      return fail("f3r_view_geometry: view %d: crop outside the resized image", i);
+    if (p.transpose != 0 && p.transpose != 1) return fail("f3r_view_geometry: view %d: transpose must be 0 or 1", i);
+    const long long n = static_cast<long long>(p.out_w) * p.out_h;
+    if (p.out_offset < 0 || n > static_cast<long long>(out_pixels) - p.out_offset)
+      return fail("f3r_view_geometry: view %d: outputs outside the output buffers", i);
+    if (n > max_pixels) max_pixels = static_cast<int>(n);
+  }
+  return check(f3r::launch_view_geometry(params_dev, count, max_pixels, out_pts, out_valid, out_depth,
+                                         static_cast<cudaStream_t>(stream)), "f3r_view_geometry");
+}
+
 int f3r_cast_bf16(const float* in, void* out, size_t count, void* stream) {
   if (!in || !out) return fail("f3r_cast_bf16: null operand");
   return check(f3r::launch_cast_bf16(in, out, count, static_cast<cudaStream_t>(stream)), "f3r_cast_bf16");

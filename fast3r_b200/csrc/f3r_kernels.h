@@ -220,6 +220,10 @@ cudaError_t launch_val_loss(const float* gt, const uint8_t* valid, const float* 
                             int n, float alpha, bool log1p, bool gt_scale, bool local_scale_consistent, bool has_local,
                             double* out, void* workspace, cudaStream_t stream);
 
+// ground-truth views (views.cu); params on the device, max_pixels = the largest out_w * out_h
+cudaError_t launch_view_geometry(const f3r_view_param* params, int count, int max_pixels, float* out_pts,
+                                 uint8_t* out_valid, float* out_depth, cudaStream_t st);
+
 // viewer scene (scene.cu)
 size_t sky_mask_workspace(int frames, int h, int w);
 cudaError_t launch_sky_mask(const float* img, int frames, int h, int w, int upper, int min_sky, int8_t* not_sky,

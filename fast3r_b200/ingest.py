@@ -81,18 +81,33 @@ def _h2d(arr: np.ndarray, device) -> torch.Tensor:
 def ingest_rgb8(img_u8: torch.Tensor, size: int = 512, square_ok: bool = False, out: torch.Tensor = None):
     """img_u8: CUDA uint8 (h, w, 3) RGB.  Returns (fp32 (3, H, W) in [-1, 1], (H, W)): resize + crop + normalise of
     load_images()."""
-    if img_u8.dtype != torch.uint8 or img_u8.dim() != 3 or img_u8.shape[2] != 3:
-        raise RuntimeError("ingest_rgb8 needs a CUDA uint8 (h, w, 3) tensor (there is no CPU path)")
-    _need_cuda(img_u8.device, "ingest_rgb8 needs a CUDA uint8 (h, w, 3) tensor (there is no CPU path)")
-    img_u8 = img_u8.contiguous()
-    if img_u8.data_ptr() % 4:  # e.g. a row slice of an image whose width is not a multiple of 4; the library needs 4
-        img_u8 = img_u8.clone()
+    _check_rgb8(img_u8)
     h1, w1, _ = img_u8.shape
     if size == 224:
         nw, nh, filt = resize_plan(w1, h1, round(size * max(w1 / h1, h1 / w1)))
     else:
         nw, nh, filt = resize_plan(w1, h1, size)
     left, top, right, bottom = crop_box(nw, nh, size, square_ok)
+    out = resize_crop_rgb8(img_u8, nw, nh, filt, (left, top, right, bottom), out)
+    return out, (bottom - top, right - left)
+
+
+def _check_rgb8(img_u8: torch.Tensor):
+    if img_u8.dtype != torch.uint8 or img_u8.dim() != 3 or img_u8.shape[2] != 3:
+        raise RuntimeError("ingest_rgb8 needs a CUDA uint8 (h, w, 3) tensor (there is no CPU path)")
+    _need_cuda(img_u8.device, "ingest_rgb8 needs a CUDA uint8 (h, w, 3) tensor (there is no CPU path)")
+
+
+def resize_crop_rgb8(img_u8: torch.Tensor, nw: int, nh: int, filt: int, box, out: torch.Tensor = None) -> torch.Tensor:
+    """PIL ``Image.resize((nw, nh), LANCZOS | BICUBIC)`` of the CUDA uint8 (h, w, 3) RGB image, then ``crop(box)`` (box =
+    (left, top, right, bottom) inside the resized image) and ToTensor + Normalize(0.5, 0.5): fp32 (3, bottom - top,
+    right - left) in [-1, 1], into `out` when given.  A dimension that keeps its size is not resampled, as in Pillow."""
+    _check_rgb8(img_u8)
+    img_u8 = img_u8.contiguous()
+    if img_u8.data_ptr() % 4:  # e.g. a row slice of an image whose width is not a multiple of 4; the library needs 4
+        img_u8 = img_u8.clone()
+    h1, w1, _ = img_u8.shape
+    left, top, right, bottom = box
     cw, ch = right - left, bottom - top
     dev = img_u8.device
     if out is None:
@@ -108,7 +123,7 @@ def ingest_rgb8(img_u8: torch.Tensor, size: int = 512, square_ok: bool = False, 
     p = ops._ptr
     ops._call("f3r_ingest_rgb8", img_u8, p(img_u8), h1, w1, nh, nw, p(hb), p(hk), hks, span, p(vb), p(vk), vks, p(tmp),
               left, top, cw, ch, p(out))
-    return out, (ch, cw)
+    return out
 
 
 def _landscape_crop(width: int, height: int):

@@ -58,6 +58,13 @@ PM_HIST, PM_MAX_BINS = 8, 64
 PM_COUNTS = PM_HIST + PM_MAX_BINS
 
 
+# f3r_view_param of f3r_view_geometry (one (view, item) of fast3r_b200.views), as a numpy record
+VIEW_PARAM = np.dtype([("depth", "<u8"), ("out_offset", "<i8"), ("src_w", "<i4"), ("src_h", "<i4"), ("crop_x", "<i4"),
+                       ("crop_y", "<i4"), ("crop_w", "<i4"), ("crop_h", "<i4"), ("rs_w", "<i4"), ("rs_h", "<i4"),
+                       ("box_x", "<i4"), ("box_y", "<i4"), ("out_w", "<i4"), ("out_h", "<i4"), ("transpose", "<i4"),
+                       ("reserved", "<i4"), ("k", "<f4", (4,)), ("pose", "<f4", (12,))])
+
+
 class JpegInfo(C.Structure):
     _fields_ = [("status", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("components", C.c_int32),
                 ("h_samp", C.c_int32), ("v_samp", C.c_int32), ("restart_interval", C.c_int32), ("segments", C.c_int32),
@@ -140,6 +147,7 @@ _API = {
     "f3r_ply_pack": (C.c_int, [_P, _P, _SIZE, _P, _P]),
     "f3r_extent_percentiles_workspace": (_SIZE, []),
     "f3r_extent_percentiles": (C.c_int, [_P, _SIZE, _SIZE, _SIZE, _F32, _F32, _P, _P, _SIZE, _P]),
+    "f3r_view_geometry": (C.c_int, [_P, _P, _I32, _P, _P, _P, _SIZE, _P]),
 }
 EXPORTS = list(_API)
 

@@ -544,6 +544,23 @@ def val_loss(gt: torch.Tensor, valid: torch.Tensor, pr: torch.Tensor, conf: torc
     return out
 
 
+# ------------------------------------------------------------------ ground-truth views (csrc/views.cu)
+def view_geometry(params: np.ndarray, out_pts: torch.Tensor, out_valid: torch.Tensor, out_depth: torch.Tensor) -> None:
+    """f3r_view_geometry over the records `params` (numpy lib.VIEW_PARAM, one per (view, item), depth pointers on the
+    device): the depth map, world points and validity of every view into the flat outputs out_pts float32 [P, 3],
+    out_valid uint8 [P] and out_depth float32 [P].  The records are checked on the host and uploaded through pinned
+    staging."""
+    if params.dtype != L.VIEW_PARAM or params.ndim != 1 or not params.flags.c_contiguous:
+        raise TypeError("view_geometry: params must be a contiguous 1-d lib.VIEW_PARAM array")
+    _chk(out_pts, F32, "out_pts"); _chk(out_valid, torch.uint8, "out_valid"); _chk(out_depth, F32, "out_depth")
+    n = out_valid.numel()
+    assert out_pts.shape == (n, 3) and out_depth.numel() == n
+    host = torch.from_numpy(params.view(np.uint8)).pin_memory()
+    dev = host.to(out_pts.device, non_blocking=True)
+    _call("f3r_view_geometry", out_pts, params.ctypes.data, _ptr(dev), len(params), _ptr(out_pts), _ptr(out_valid),
+          _ptr(out_depth), n)
+
+
 # ------------------------------------------------------------------ viewer scene (csrc/scene.cu)
 I8, U8 = torch.int8, torch.uint8
 

@@ -397,6 +397,36 @@ size_t f3r_extent_percentiles_workspace(void);
 int f3r_extent_percentiles(const float* pts, size_t n, size_t k0, size_t k1, float g0, float g1, float* out,
                            void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- ground-truth views: the depth half of the datasets' principal-point crop, rescale and crop
+ * (fast3r/dust3r/datasets/base/base_stereo_view_dataset.py:165-221), the unprojection to world points
+ * (fast3r/dust3r/utils/geometry.py:186-243), the validity mask and the landscape transpose (:78-142, :243-261).  The host
+ * plans the geometry and runs the image half through f3r_ingest_rgb8 (fast3r_b200/views.py).
+ *
+ * One f3r_view_param per (view, item).  The depth map depth [src_h][src_w] (DEVICE, float32) is cropped to the box
+ * (crop_x, crop_y, crop_w, crop_h), resized to (rs_w, rs_h) with cv2's INTER_NEAREST rule and cropped to (box_x, box_y,
+ * out_w, out_h).  Pixel (u, v) of that crop at depth z has the camera point ((u - k[2]) z / k[0], (v - k[3]) z / k[1], z)
+ * (in float64, rounded to float32) and the world point pose[0..11] = [R | t] (row-major) applied in float32; it is
+ * valid when z > 0 and the world point is finite (a NaN pose makes every pixel invalid).  Pixel i of the view's outputs
+ * is element out_offset + i of out_pts [.][3], out_valid (uint8 0/1) and out_depth; the outputs are stored row-major as
+ * [out_h][out_w], or transposed as [out_w][out_h] when transpose = 1. */
+typedef struct f3r_view_param {
+  const float* depth;
+  int64_t out_offset;
+  int32_t src_w, src_h;
+  int32_t crop_x, crop_y, crop_w, crop_h;
+  int32_t rs_w, rs_h;
+  int32_t box_x, box_y, out_w, out_h;
+  int32_t transpose, reserved;
+  float k[4];     /* fu, fv, cu, cv of the final intrinsics */
+  float pose[12]; /* cam2world rows [R | t] */
+} f3r_view_param;
+
+/* f3r_view_geometry: params (HOST) is checked before any CUDA call - every box inside its image, depth 4-byte
+ * aligned, every view's outputs inside [0, out_pixels), out_pixels and every source below 2^31 pixels, 1 <= count <=
+ * 65535 - and params_dev holds the same count records on the DEVICE, which the kernel reads.  One launch. */
+int f3r_view_geometry(const f3r_view_param* params, const f3r_view_param* params_dev, int32_t count, float* out_pts,
+                      uint8_t* out_valid, float* out_depth, size_t out_pixels, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
